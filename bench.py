@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- SAVP training hot path on B200 (frames/sec, BASELINE.json metric).
+"""bench.py -- SAVP training hot path on H100 (frames/sec, BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run, one rank per GPU)
   python bench.py --impl reference ...                      (the CPU arm: the oracle port on the host cores)
+  python bench.py ... --dump-outputs DIR                    (also writes what the last timed step computed, as .npy files)
 
 A "step" is one full optimisation step of --config (default cfg2 = configs[1] of BASELINE.json: SAVP, bair_action_free/ours_savp
 hparams: VAE+GAN, 64x64x3, 2 context + 10 predicted, batch 16 per GPU): generator forward (posterior + prior unrolls),
@@ -14,6 +15,8 @@ frames/sec = global_batch * (T-1) generated frames per step / step time.
             inside the timed region.
 `roofline`: the ConvLSTM gate convolutions (rnn_ops.py:121; the north-star kernel) timed alone with CUDA events, and
             `roofline.whole_engine`: every tensor-core call of one step (forward + dgrad + wgrad).
+Inputs, parameter initialisation and per-step noise are seeded, so two runs with the same arguments feed identical inputs
+and --dump-outputs files of two builds can be compared array by array.
 """
 from __future__ import annotations
 
@@ -54,7 +57,7 @@ CONFIGS = {
                  image=(64, 64, 1), actions=0, batch=32),
 }
 CFG = CONFIGS['cfg2']
-SAVP_HPARAMS = CFG['hparams']          # kept for tests/profile_step.py
+SAVP_HPARAMS = CFG['hparams']
 IMAGE = CFG['image']
 PER_GPU_BATCH = CFG['batch']
 
@@ -70,7 +73,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d['hbm_gbs'], bf16=d['bf16_tflops'], bf16_sustained=d.get('bf16_tflops_sustained'), src='measured')
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src='fallback')
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- a ceiling, not a measured rate
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=None, src='H100 SXM data sheet')
 
 
 class ClockSampler(threading.Thread):
@@ -181,32 +185,6 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-def ncu_traffic():
-    """DRAM traffic of the dominant kernel per launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed
-    `ncu --set full` capture of the lstm_h0 gate convolution (profiles/r02_ncu_full_summary.json, tests/ncu_capture_r02.sh),
-    next to the algorithmic bytes of that launch (input + packed weights read, gate pre-activations written)."""
-    out = dict(traffic=None)
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'r02_ncu_full_summary.json')
-
-    def mb(v):
-        num, unit = v.split()[:2]
-        return float(num) * {'byte': 1.0, 'Kbyte': 1e3, 'Mbyte': 1e6, 'Gbyte': 1e9}[unit]
-    try:
-        with open(path) as f:
-            caps = json.load(f)['captures']['r02_engine_kernels.ncu-rep']
-        c = [x for x in caps if 'igemm_halo' in x['kernel'] and x['grid'].startswith('(128,')][0]   # lstm_h0: 128 M = 256 tiles
-        out['traffic'] = mb(c['dram_bytes_read']) + mb(c['dram_bytes_write'])
-        out['traffic_unit'] = 'bytes per launch (lstm_h0 gate conv, halo mode, ncu --set full)'
-        out['traffic_algorithmic'] = 32 * 1024 * 72 * 4 + 25 * 128 * 96 * 4 + 32 * 1024 * 128 * 4
-        out['traffic_note'] = ('reads = input + weights once (no re-reads from HBM); the 16.8 MB of gate pre-activations stay in the '
-                               '126 MB L2 for the gate kernel that follows, so almost nothing is written back')
-        out['tensor_pipe_active_pct'] = float(c['tensor_pipe_active_pct_of_active'].split()[0])
-        out['l2_to_sm_bytes'] = mb(c['l1tex__m_xbar2l1tex_read_bytes.sum'])
-    except Exception:       # noqa: BLE001  (profile summary absent: leave traffic null)
-        pass
-    return out
-
-
 def time_gate_kernels(model, iters=3):
     """CUDA-event timing of the five ConvLSTM gate convolutions (one launch per timestep buffer, cycling through all
     T-1 timesteps so consecutive launches touch different HBM lines; working set > L2), replayed from a CUDA graph."""
@@ -223,7 +201,7 @@ def time_gate_kernels(model, iters=3):
         for t in range(S):
             conv.fwd(rin[t], gpre[t])
         torch.cuda.synchronize()
-        # the S launches are replayed from a CUDA graph: a 16 us kernel launched eagerly through ctypes is host-bound
+        # the S launches are replayed from a CUDA graph: a kernel of a few microseconds launched eagerly through ctypes is host-bound
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             for t in range(S):
@@ -297,6 +275,35 @@ def engine_profile(model, batch):
             os.environ['VP_CONCURRENT_D'] = old
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(model, out_dir):
+    """What the caller of the timed path receives from its last step: the loss terms (float64, model.losses()), the frames the
+    step's generator produced (the time-major device buffer behind outputs['gen_images']) and the updated variables, as
+    DIR/<name>.npy.  Arrays over the per-array cap are replaced by a fixed, seeded sample of their elements (flattened) so
+    that the files stay under 64 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    losses = model.losses()
+    for k, v in losses.items():
+        np.save(os.path.join(out_dir, 'loss.%s.npy' % k), np.array([v], dtype=np.float64))
+    # the captured step runs the generator without collecting model.outputs; its frames are in the buffer the graph writes
+    arrays = {'gen_images': model.outputs_time_major('gen_images').float().cpu().numpy()}
+    if arrays['gen_images'].size == 0:
+        raise RuntimeError('--dump-outputs: the step produced no generated frames')
+    for k, v in model.get_params().items():
+        arrays['param.' + k.replace('/', '.')] = v.astype(np.float32)
+    budget = DUMP_LIMIT_BYTES - 64 * 1024
+    per_array = max(4096, budget // max(1, len(arrays)))
+    rng = np.random.default_rng(0)
+    for name, a in arrays.items():
+        if a.nbytes > per_array:
+            idx = np.sort(rng.choice(a.size, per_array // 4, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -330,7 +337,7 @@ def run_ours(args):
     if world > 1:
         dist.barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    k_e2e = max(3, min(args.steps, 10))
+    k_e2e = args.steps
     t0 = time.time()
     e0.record()
     for i in range(k_e2e):
@@ -383,6 +390,9 @@ def run_ours(args):
         dist.barrier()
     losses = model.losses()
     finite = all(v == v for v in losses.values())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(model, args.dump_outputs)
+        log('outputs of the last timed step written to %s' % args.dump_outputs)
 
     # ---------------- rooflines + CPU baseline (rank 0; the CPU leg at N = 1 only)
     no_engine_ms = None
@@ -397,11 +407,11 @@ def run_ours(args):
             flops, gate_ms, per_layer = time_gate_kernels(model)
             log('gate kernels timed; cpu baseline leg')
             achieved = flops / gate_ms / 1e9     # TFLOP/s over the gate convolutions of one timestep
-            roof = dict(bound='tensor', kernel='ConvLSTM gate convolutions (rnn_ops.py:121) on the tcgen05 kind::tf32 engine, forward',
+            roof = dict(bound='tensor', kernel='ConvLSTM gate convolutions (rnn_ops.py:121) on the wgmma TF32 engine, forward',
                         achieved=achieved, peak=peaks['bf16'], unit='TFLOP/s', frac=achieved / peaks['bf16'],
-                        peak_source=peaks['src'] + ' cuBLAS bf16 (burst); the tf32 MMA rate is half of bf16',
+                        peak_source=peaks['src'] + ' bf16; the tf32 MMA rate is half of bf16',
                         peak_tf32_equiv=peaks['bf16'] / 2, frac_of_tf32_peak=achieved / (peaks['bf16'] / 2),
-                        per_layer=per_layer, **ncu_traffic())
+                        per_layer=per_layer)
             tot_f = sum(d['flops'] for d in prof.values())
             tot_ms = sum(d['ms'] for d in prof.values())
             sustained = (peaks.get('bf16_sustained') or peaks['bf16']) / 2
@@ -442,7 +452,7 @@ def run_ours(args):
                                          'post-update D fwd + G BPTT + Adam(G)' % (CFG['what'], B), name=args.config,
                                 global_batch=world * B, per_gpu_batch=B, sequence_length=SAVP_HPARAMS['sequence_length'],
                                 parallelism='dp%d' % world, cuda_graph=graph is not None,
-                                l2='working set of one step (GBs of activations) is far larger than the 126 MB L2'),
+                                l2='working set of one step (GBs of activations) is far larger than the 50 MB L2'),
                     e2e=dict(value=frames_per_step / e2e_ms * 1e3, unit='frames/s', ms_per_step=e2e_ms, h2d_bytes_per_step=h2d,
                              d2h_bytes_per_step=d2h, api='get_model_class("savp")(...).train_step(host inputs) + .losses()'),
                     gpu_launches=int(launches_per_step) * args.steps, gpu_launches_per_step=int(launches_per_step),
@@ -473,13 +483,15 @@ def main():
     faulthandler.dump_traceback_later(int(os.environ.get('BENCH_WATCHDOG_S', '420')), exit=True)   # a hang dumps all stacks and exits
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=20)
+    ap.add_argument('--steps', type=int, default=20, help='timed steps of the graph-replayed loop (value) and of the e2e loop')
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--no-graph', action='store_true')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-roofline', action='store_true', help='skip the roofline legs (gate kernels, whole-engine profile)')
     ap.add_argument('--config', default='cfg2', choices=sorted(CONFIGS), help='BASELINE.json configs[i-1]; the metric is quoted on cfg2')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the losses, generated frames and updated variables of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
     select_config(args.config)
     if args.impl == 'reference':

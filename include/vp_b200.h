@@ -1,5 +1,5 @@
 /*
- * vp_b200.h -- C ABI of libvp_b200.so: the B200 (sm_100a) kernels behind the SAVP training path.
+ * vp_b200.h -- C ABI of libvp_b200.so: the H100 (sm_90a) kernels behind the SAVP training path.
  *
  * The reference (alexlee-gk/video_prediction) has no FFI: its seam is the Python model registry
  * (video_prediction/models/__init__.py:12-25) whose classes call tf.nn.* primitives.  Each entry
@@ -51,28 +51,20 @@ enum { VP_WLAYOUT_FWD = 0, VP_WLAYOUT_DGRAD = 1,
        VP_WLAYOUT_RESIDUAL = 4 /* OR-ed in: pack tf32(w - tf32(w)), the low part of the fp32-exact 3xTF32 mode */ };
 
 const char* vp_last_error(void);
-/* debug: per-CTA globaltimer stamps of the last vp_conv_igemm launch made with VP_FWD_TRACE=1 (8 x u64 per CTA) */
-int vp_debug_read_trace(unsigned long long* host, int n_ctas);
 int vp_version(void);
 
-/* ---- tensor-core implicit-GEMM convolution (tcgen05 / TMEM / TMA) ------------------------------
+/* ---- tensor-core implicit-GEMM convolution (wgmma / mma.sync / TMA) -----------------------------
  * Replaces tf.nn.conv2d (rnn_ops.py:121, ops.py:528), tf.nn.conv2d_transpose (ops.py:584),
  * tf.nn.conv3d (ops.py:773) and their gradients.
  * wpacked: [kd*kh*kw][n_pad][kc*32] floats (see vp_pack_weights); GEMM N = n_pad (multiple of 16),
  * GEMM K = kc 32-channel chunks of in->c per tap.  out->c columns are stored.
  * split_k > 1: partial sums are atomically added into `out` (caller zero-fills; act must be NONE;
- * bias is added by split 0).  split_k == 0: automatic -- an under-filled grid with a long K loop is split and a DENSE
- * output (out->c == out->cstride) is cleared by the call itself.  accumulate = 1: out += result (act must be NONE);
+ * bias is added by split 0), so the fp32 result depends on the order the splits finish in.  split_k == 0 and 1: unsplit
+ * (run-to-run identical results).  accumulate = 1: out += result (act must be NONE);
  * accumulate = 2: out = act(out + result + bias) -- the last pass of a multi-pass (3xTF32) accumulation. */
 int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
                   const vp_tensor* out, const float* bias, int act, float alpha, int split_k, int accumulate,
                   vp_stream_t stream);
-
-/* Engine selection for vp_conv_igemm / vp_conv_igemm_actgrad on the calling thread: 0 = box mode (one activation tile per
- * filter tap), 1 = halo mode (one halo tile per tap group, 256 output positions per CTA; falls back to box mode when the
- * geometry is not eligible), -1 = default (halo unless the environment says VP_HALO=0).  Both engines compute the same
- * sums (fp32 summation order differs); the host layer times both once per geometry and keeps the faster. */
-int vp_conv_set_engine(int engine);
 
 /* Input-gradient convolution fused with the backward of the previous layer's activation:
  *   out = (conv(in) + addend) * act'(act_output),  act' evaluated from the activation OUTPUT (lrelu/relu/sigmoid/tanh);
@@ -267,9 +259,10 @@ int vp_conv3d_c4_fwd(const float* x, const float* w, const float* inv_scale, con
                      int h, int wd, int ci, float lrelu_alpha, vp_stream_t stream);
 int vp_conv3d_c4_wgrad(const float* x, const float* dy, float* gw, int n, int d, int h, int wd, int ci, vp_stream_t stream);
 /* The same layer on the tensor cores (TF32 operands, fp32 accumulate), without repacking x (csrc/d0_layer.cu):
- *  fwd:   a flat halo tile of float4 voxels is the un-swizzled K-major operand; the next-voxel leading offset (LBO = 16 B)
- *         turns x[v-1 .. v+2] into the K = 16 operand of one kernel row.  Needs h % 4 == 0 and a tile that fits (64^2, 128^2 do).
- *  wgrad: rows of float4 voxels are the 32-byte-atom MN-major operand, dy arrives phase-major.  Needs wd % 64 == 0. */
+ *  fwd:   a flat halo tile of float4 voxels is the un-swizzled K-major wgmma operand; the next-voxel leading offset
+ *         (LBO = 16 B) turns x[v-1 .. v+2] into the K = 16 operand of one kernel row.  Needs h % 4 == 0 and a tile that fits
+ *         (64^2, 128^2 do).
+ *  wgrad: the overlapping float4 voxels of a halo row are the (dx, ci) x voxel operand of mma.sync.  Needs wd % 64 == 0. */
 int vp_conv3d_c4_fwd_tc(const float* x, const float* w, const float* inv_scale, const float* bias, float* out, int n, int d, int h,
                         int wd, int ci, float lrelu_alpha, vp_stream_t stream);
 int vp_conv3d_c4_wgrad_tc(const float* x, const float* dy, float* gw, int n, int d, int h, int wd, int ci, vp_stream_t stream);
@@ -278,12 +271,6 @@ int vp_gather_clip(const float* video, const int32_t* t_start, float* clip, int 
                    int video_batch, int batch_offset, vp_stream_t stream);
 int vp_scatter_clip(const float* dclip, const int32_t* t_start, float* dvideo, int clips, int clip_len, long long pixels,
                     int video_batch, int batch_offset, vp_stream_t stream);
-
-/* Debug: one tcgen05.mma kind::tf32 (M = 128, N = n, K = 8) on caller-supplied shared-memory images and descriptor fields
- * (start offset, LBO, SBO in bytes; layout type 0 none, 1 = 128B/32B-atom, 2 = 128B; major 0 = K, 1 = MN).  out = [128][n]. */
-int vp_debug_umma_probe(const void* a_img, int a_bytes, const void* b_img, int b_bytes, unsigned a_start, unsigned a_lbo,
-                        unsigned a_sbo, unsigned a_layout, int a_mn_major, unsigned b_start, unsigned b_lbo, unsigned b_sbo,
-                        unsigned b_layout, int b_mn_major, int n, float* out, vp_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -15,7 +15,7 @@ conv dgrad, fused_batch_norm training-mode biased variance, TF1 Adam).  It is pi
 
 Layout conventions follow the reference: activations NHWC / NDHWC, time-major [T,B,...] inside
 the path, conv filters HWIO, conv2d_transpose filters [kh,kw,Cout,Cin].  Every function cites the
-reference file:line it restates (paths relative to /root/reference/video_prediction/).
+reference file:line it restates (paths relative to the reference's video_prediction/ package).
 
 All randomness (weights, eps, prior z, scheduled-sampling mask, discriminator clip offsets) is an
 explicit input so that the CUDA path and the oracle see identical numbers.
@@ -99,8 +99,8 @@ def _nhwc(x):
 
 
 # ---- optional emulation of the CUDA path's tensor-core arithmetic --------------------------------
-# The sm_100a engine feeds fp32 operands to tcgen05.mma kind::tf32, which reads only the top 19 bits
-# of each operand (sign, 8 exponent, 10 mantissa bits) and accumulates in fp32.  With
+# The sm_90a engine feeds fp32 operands to the TF32 tensor-core MMAs, which read only the top 19 bits
+# of each operand (sign, 8 exponent, 10 mantissa bits) and accumulate in fp32.  With
 # `set_tf32_emulation('trunc')` every convolution of the oracle (forward AND its autograd backward:
 # dgrad sees tf32(dy) x tf32(W), wgrad sees tf32(x) x tf32(dy)) quantises its operands the same way, so a
 # difference between the CUDA path and this oracle that is NOT explained by operand rounding shows up

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Evaluation driver with the reference's command line (scripts/evaluate.py:143-175 of alexlee-gk/video_prediction) on the B200
+"""Evaluation driver with the reference's command line (scripts/evaluate.py:143-175 of alexlee-gk/video_prediction) on the H100
 SAVP path: for every batch of the val / test split, `num_stochastic_samples` predictions are drawn and the best / average /
 worst one per video is kept for every metric (base_model.py:132-227 -> `model.eval_outputs_and_metrics`), written in the
 reference's result layout

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Sampling driver with the reference's command line (scripts/generate.py:19-49) on the B200 SAVP path: restores a
+"""Sampling driver with the reference's command line (scripts/generate.py:19-49) on the H100 SAVP path: restores a
 checkpoint written by scripts/train.py, runs the generator in test mode (prior unroll, no discriminators) for
 `--num_stochastic_samples` noise draws per batch, and writes the predicted future frames as PNGs
 (`gen_image_%05d_%02d_%02d.png`, generate.py:183-190) and, per sample, the context + future frames as an animated GIF

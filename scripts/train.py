@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Training driver with the reference's command line (scripts/train.py:30-61 of alexlee-gk/video_prediction) on the B200
+"""Training driver with the reference's command line (scripts/train.py:30-61 of alexlee-gk/video_prediction) on the H100
 SAVP path.  Same flags, same options.json / dataset_hparams.json / model_hparams.json side files, same progress print-out
 (global step, image/sec, d_loss / g_loss and their terms, learning rate), same checkpoint cadence -- no TensorFlow:
 `sess.run(train_op)` becomes `model.train_step(batch)`.

@@ -1,6 +1,6 @@
 """Timing ablation of the cfg2 training step: the step is re-captured with one kernel family not launched (VP_SKIP, results
 are wrong by design) and the difference to the full step is that family's REAL cost inside the CUDA graph (warm L2, overlap
-with the parallel branches) -- unlike the ncu launch list, whose per-launch times are cold-cache and serialised."""
+with the parallel branches), which per-launch timings (cold caches, serialised) do not show."""
 import json
 import os
 import subprocess

@@ -2,7 +2,7 @@
 2 context + 10 predicted frames) and of the 30-frame cfg3 shape with the convolution operands quantised as a tensor core
 would read them -- TF32 as the CUDA path does (activations truncated, weights rounded to nearest) and bf16 (what kind::f16
 operands would see) -- against the un-quantised fp32 oracle.  The contract is 1e-3 max-abs on images in [0, 1].
-Usage: python tests/measure_bf16_tolerance.py > profiles/r02_bf16_vs_tf32_tolerance.log"""
+Usage: python tests/measure_bf16_tolerance.py"""
 import os
 import sys
 

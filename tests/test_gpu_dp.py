@@ -56,8 +56,7 @@ def _worker(rank, world, port, q, env):
 
 @pytest.mark.parametrize('mode,buckets,tol', [('exact', '0', 3e-3), ('tf32', '1', 2e-2)])
 def test_two_ranks_equal_one_rank_on_the_global_batch(mode, buckets, tol):
-    """exact: fp32-exact convolutions (VP_EXACT=1) -> the two runs differ by fp32 summation order only (3e-3, see
-    profiles/r02_parity_noise_floor.md).  tf32: product arithmetic, where different tile / split-K decisions at B/2 flip
+    """exact: fp32-exact convolutions (VP_EXACT=1) -> the two runs differ by fp32 summation order only.  tf32: product arithmetic, where different tile / split-K decisions at B/2 flip
     operand truncations downstream (two correct TF32 runs differ by ~0.5 %); this variant also exercises the bucketed,
     overlapped all-reduce (VP_DP_BUCKETS=1)."""
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:

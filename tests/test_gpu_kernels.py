@@ -337,7 +337,7 @@ def test_conv3d_c4_cuda_core_first_discriminator_layer(L):
 
 @pytest.mark.parametrize('N,D,H,W,C', [(2, 3, 5, 64, 3), (1, 2, 3, 128, 1), (3, 10, 64, 64, 3)])
 def test_conv3d_c4_wgrad_tensor_cores(L, N, D, H, W, C):
-    """vp_conv3d_c4_wgrad_tc (float4 voxel rows as the un-swizzled MN-major UMMA operand, one MMA per dx) against the fp64
+    """vp_conv3d_c4_wgrad_tc (the overlapping float4 voxels of a halo row as the (dx, ci) x voxel mma.sync operand) against the fp64
     weight gradient of the operands the tensor core reads (fp32 truncated to TF32), and against the CUDA-core kernel."""
     def trunc(t):
         return (t.contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32)

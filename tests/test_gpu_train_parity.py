@@ -1,7 +1,7 @@
 """GPU parity tests (-m gpu) of the TRAINING step and of the full-length BASELINE configurations against the CPU oracle
 in plain fp32 (the reference's arithmetic), in the two arithmetic modes of the CUDA path:
 
-  * product mode: TF32 tensor-core operands (activations truncated by tcgen05, weights rounded when packed), fp32
+  * product mode: TF32 tensor-core operands (activations truncated by the tensor cores, weights rounded when packed), fp32
     accumulation.  Generator outputs 1e-3 max-abs (BASELINE.json north_star); model-level gradients 5e-2 relative L2 per
     tensor (operand rounding through an 11-step BPTT and a 7-layer discriminator is 1-3 % on the largest tensors).
   * fp32-exact mode (VP_EXACT=1): every tensor-core convolution as three TF32 passes hi*hi + lo*hi + hi*lo.  Here every
@@ -12,7 +12,7 @@ in plain fp32 (the reference's arithmetic), in the two arithmetic modes of the C
 Why not an oracle with TF32-quantised operands for the model-level gradients?  It exists (`O.set_tf32_emulation`, used by the
 op-level tests in test_gpu_kernels.py at 1e-5) but operand truncation is discontinuous: fp32 summation-order noise upstream
 flips quantisation decisions downstream, so two correct TF32 implementations differ by 0.5-1.5 % on these gradients
-(measured: the emulating oracle with fp32 vs fp64 accumulation, profiles/r02_parity_noise_floor.md).
+(measured: the emulating oracle with fp32 vs fp64 accumulation).
 """
 import os
 import sys
@@ -40,7 +40,7 @@ _MODE = {}
 
 
 def tf32_mode():
-    """Which quantisation the tensor cores apply to fp32 operands of kind::tf32: measured, not assumed."""
+    """Which quantisation the tensor cores apply to fp32 operands of the TF32 MMAs: measured, not assumed."""
     if 'mode' in _MODE:
         return _MODE['mode']
     from video_prediction_b200 import lib as L
@@ -66,7 +66,7 @@ def tf32_mode():
 
 def test_tensor_core_operand_quantisation_is_identified():
     mode = tf32_mode()
-    print('tcgen05 kind::tf32 operand quantisation:', mode, _MODE['errs'])
+    print('TF32 tensor-core operand quantisation:', mode, _MODE['errs'])
     assert mode in ('trunc', 'rna')
 
 
@@ -144,9 +144,8 @@ CASES = {
 MODES = {'tf32': ('0', 1e-2, 1e-3, 1e-3), 'exact': ('1', 2e-3, 1e-4, 1e-4)}   # (post-update D features follow +-lr Adam steps)
 # fp32-exact mode: relative-L2 bound per gradient tensor.  Generator-only cases: 2e-3 (3x the oracle's own fp32-vs-fp64 noise).
 # With the discriminators the gradient is a near-cancellation of the real and the fake clip's contributions and the tensor
-# core's fp32 accumulator is ~10x less accurate than a CPU fp32 convolution (profiles/r02_exact_mode_accumulator.log: error
-# proportional to K, 1.4e-5 at K = 6400): 1e-2 for the shipped LSGAN configuration (measured 4.7e-3 ... 7.5e-3 depending on the
-# engines' summation order; 3.3e-3 at B=16).  'savp_gan_l2' starts with logits ~ 0
+# core's fp32 accumulator is less accurate than a CPU fp32 convolution (its error grows with K): 1e-2 for the shipped LSGAN
+# configuration.  'savp_gan_l2' starts with logits ~ 0
 # under the sigmoid-CE loss, where the real/fake terms cancel to 1 % (the CPU fp32 oracle itself is 5e-3 from fp64 there).
 EXACT_GTOL = {'deterministic_l1': 2e-3, 'vae_l1': 2e-3, 'vae_flow': 3e-3, 'savp': 1e-2, 'image_video_gan': 1e-2, 'savp_gan_l2': 5e-2}
 
@@ -333,8 +332,7 @@ def test_captured_step_reproduces_the_eager_step(Model, tmp_path):
     """The step bench.py times is ONE captured CUDA graph with parallel branches (discriminator towers, spectral norm + packing
     under the generator forward).  From the same checkpoint and batch: the eager step, a captured replay and a second replay
     must produce the same losses and gradients up to what summation-order noise becomes in TF32 arithmetic (atomics in split-K
-    and the weight gradients reorder fp32 sums; downstream truncations to TF32 flip, profiles/r02_parity_noise_floor.md):
-    measured 7e-4 / 1e-3 between two replays and 9e-3 / 3e-3 between the graph and the eager step (G / D gradients).  A step
+    and the weight gradients reorder fp32 sums; downstream truncations to TF32 flip).  A step
     that is not executed at capture time (the bug this test found), a stale buffer or a race between branches shows as O(1)."""
     import make_golden_b16 as G
     hp, params, inputs, noise = G.case()

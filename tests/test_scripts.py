@@ -25,10 +25,10 @@ def test_train_and_generate_accept_the_reference_argument_set(tmp_path):
     import train
     import generate
     flags = {a.option_strings[0]: a for a in train.build_parser()._actions if a.option_strings}
-    assert set(REFERENCE_TRAIN_FLAGS) <= set(flags)                          # /root/reference/scripts/train.py:30-61
+    assert set(REFERENCE_TRAIN_FLAGS) <= set(flags)                          # the reference's scripts/train.py:30-61
     assert flags['--summary_freq'].default == 1000 and flags['--save_freq'].default == 5000 and flags['--progress_freq'].default == 100
     gflags = {a.option_strings[0]: a for a in generate.build_parser()._actions if a.option_strings}
-    assert set(REFERENCE_GENERATE_FLAGS) <= set(gflags)                      # /root/reference/scripts/generate.py:19-49
+    assert set(REFERENCE_GENERATE_FLAGS) <= set(gflags)                      # the reference's scripts/generate.py:19-49
     assert gflags['--batch_size'].default == 8 and gflags['--num_stochastic_samples'].default == 5 and gflags['--seed'].default == 7
     # the README's training command line (bair_action_free / ours_savp), with the synthetic dataset
     hp = tmp_path / 'model_hparams.json'
@@ -178,7 +178,7 @@ REFERENCE_EVALUATE_FLAGS = ['--input_dir', '--results_dir', '--output_dir', '--c
 def test_evaluate_accepts_the_reference_argument_set_and_writes_its_csv_layout(tmp_path):
     import evaluate
     flags = {a.option_strings[0]: a for a in evaluate.build_parser()._actions if a.option_strings}
-    assert set(REFERENCE_EVALUATE_FLAGS) <= set(flags)                       # /root/reference/scripts/evaluate.py:143-175
+    assert set(REFERENCE_EVALUATE_FLAGS) <= set(flags)                       # the reference's scripts/evaluate.py:143-175
     assert flags['--num_stochastic_samples'].default == 100 and flags['--eval_substasks'].default == ['max', 'avg', 'min']
     assert flags['--mode'].choices == ['val', 'test'] and flags['--seed'].default == 7
     with pytest.raises(ValueError):

@@ -1,7 +1,7 @@
-"""Builds libvp_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Builds libvp_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
-The .so is git-ignored but travels with the gpurun snapshot; the product path never falls back
-to anything else when it is missing (video_prediction_b200/lib.py raises)."""
+The .so and its object files are git-ignored build products; the product path never falls back
+to anything else when the library is missing (video_prediction_b200/lib.py raises)."""
 from __future__ import annotations
 
 import os
@@ -12,10 +12,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 LIB_PATH = os.path.join(HERE, 'libvp_b200.so')
-SOURCES = ['api.cu', 'igemm.cu', 'pack.cu', 'elementwise.cu', 'backward.cu', 'discrim.cu', 'planes.cu', 'd0_layer.cu', 'debug_probe.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
-              '-Xcompiler', '-fPIC', '--use_fast_math', '-Xptxas', '-v',
-              '-I', os.path.join(ROOT, 'include'), '-I', CSRC]
+SOURCES = ['api.cu', 'igemm.cu', 'pack.cu', 'elementwise.cu', 'backward.cu', 'discrim.cu', 'planes.cu', 'd0_layer.cu']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17',
+                     '-Xcompiler', '-fPIC', '--use_fast_math', '-Xptxas', '-v',
+                     '-I', os.path.join(ROOT, 'include'), '-I', CSRC]
 
 
 def _nvcc():
@@ -67,7 +68,7 @@ def build(force=False, verbose=False):
             if r.returncode:
                 raise RuntimeError('nvcc failed on %s' % s)
             objs.append(o)
-    cmd = [_nvcc(), '-shared', '-o', LIB_PATH] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [_nvcc(), '-shared', '-o', LIB_PATH] + objs + ARCH
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)

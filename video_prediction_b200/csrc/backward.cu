@@ -94,8 +94,9 @@ __global__ void __launch_bounds__(512) inorm_act_bwd_kernel(const float* __restr
   }
   bsum<8>(s, scratch);
   if (threadIdx.x < 4) {
-    atomicAdd(dbeta + c0 + threadIdx.x, s[threadIdx.x]);
-    atomicAdd(dgamma + c0 + threadIdx.x, s[4 + threadIdx.x]);
+    // per-sample partials (rows of a scratch buffer), added in sample order by vp_inorm_act_bwd
+    dbeta[static_cast<long long>(n) * C + c0 + threadIdx.x] = s[threadIdx.x];
+    dgamma[static_cast<long long>(n) * C + c0 + threadIdx.x] = s[4 + threadIdx.x];
   }
   const float inv = 1.f / P;
   float* dp = dx + static_cast<long long>(n) * P * dxs + c0;
@@ -201,8 +202,9 @@ __global__ void __launch_bounds__(512) lstm_gates_bwd_kernel(
   }
   bsum<8>(sA, scratch);
   if (threadIdx.x < 4) {
-    atomicAdd(db2 + c0 + threadIdx.x, sA[threadIdx.x]);
-    atomicAdd(dg2 + c0 + threadIdx.x, sA[4 + threadIdx.x]);
+    // per-sample partials (rows of a scratch buffer), added in sample order by vp_lstm_gates_bwd
+    db2[static_cast<long long>(n) * F + c0 + threadIdx.x] = sA[threadIdx.x];
+    dg2[static_cast<long long>(n) * F + c0 + threadIdx.x] = sA[4 + threadIdx.x];
   }
   // ---- pass B: dc' -> gate grads (w.r.t. normalised+affine gates); sums for the gate norm
   float sB[32];
@@ -247,8 +249,8 @@ __global__ void __launch_bounds__(512) lstm_gates_bwd_kernel(
   bsum<32>(sB, scratch);
   if (threadIdx.x < 16) {
     const int g = threadIdx.x >> 2, k = threadIdx.x & 3;
-    atomicAdd(db1 + g * F + c0 + k, sB[threadIdx.x]);
-    atomicAdd(dg1 + g * F + c0 + k, sB[16 + threadIdx.x]);
+    db1[static_cast<long long>(n) * 4 * F + g * F + c0 + k] = sB[threadIdx.x];
+    dg1[static_cast<long long>(n) * 4 * F + g * F + c0 + k] = sB[16 + threadIdx.x];
   }
   // ---- pass C: gate-norm backward -> dpre
   float* dpp = dpre + static_cast<long long>(n) * P * 4 * F;
@@ -303,20 +305,17 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __res
                                                              const float* __restrict__ dB, int dbs,
                                                              float* __restrict__ dimage, float* __restrict__ dkern, int N,
                                                              int H, int W, int KH, int KW, int NK) {
-  extern __shared__ float sk[];  // [KK*NK] kernels, then [KK*NK] dkern partials
+  extern __shared__ float sk[];  // [KK*NK] kernels, then [8 warps][KK*NK] dkern partials
   const int n = blockIdx.y;
   const int KK = KH * KW;
   float* sdk = sk + KK * NK;
-  for (int i = threadIdx.x; i < KK * NK; i += blockDim.x) {
-    sk[i] = kern[static_cast<long long>(n) * KK * NK + i];
-    sdk[i] = 0.f;
-  }
+  for (int i = threadIdx.x; i < KK * NK; i += blockDim.x) sk[i] = kern[static_cast<long long>(n) * KK * NK + i];
+  for (int i = threadIdx.x; i < 8 * KK * NK; i += blockDim.x) sdk[i] = 0.f;
   __syncthreads();
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   const bool valid = p < H * W;
   const int y = valid ? p / W : 0, x = valid ? p % W : 0;
   const float4* img = image + static_cast<long long>(n) * H * W;
-  float* dimg = dimage + static_cast<long long>(n) * H * W * 4;
   float4 dT[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -328,39 +327,73 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __res
       dT[k] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
     }
   }
-  if (valid) {  // prev-image background layer (slot NK) passes its gradient straight to the image
-    const long long o = (static_cast<long long>(n) * H * W + p);
-    const float4 a = *reinterpret_cast<const float4*>(dA + o * das + 4 * NK);
-    const float4 b = *reinterpret_cast<const float4*>(dB + o * dbs + 4 * NK);
-    atomicAdd(dimg + p * 4 + 0, a.x + b.x); atomicAdd(dimg + p * 4 + 1, a.y + b.y);
-    atomicAdd(dimg + p * 4 + 2, a.z + b.z);
-  }
   const int ph = (KH - 1) / 2, pw = (KW - 1) / 2;
-  const int lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int i = 0; i < KH; ++i) {
     const int yy = reflect_i(y + i - ph, H);
     for (int j = 0; j < KW; ++j) {
       const int xx = reflect_i(x + j - pw, W);
       const int q = yy * W + xx;
       const float4 v = valid ? img[q] : make_float4(0.f, 0.f, 0.f, 0.f);
-      const float* kk = sk + (i * KW + j) * NK;
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         if (k < NK) {
-          acc.x += kk[k] * dT[k].x; acc.y += kk[k] * dT[k].y; acc.z += kk[k] * dT[k].z;
           float d = dT[k].x * v.x + dT[k].y * v.y + dT[k].z * v.z + dT[k].w * v.w;
           d = wsum(d);
-          if (lane == 0) atomicAdd(&sdk[(i * KW + j) * NK + k], d);
+          if (lane == 0) sdk[warp * KK * NK + (i * KW + j) * NK + k] += d;
         }
-      }
-      if (valid) {
-        atomicAdd(dimg + q * 4 + 0, acc.x); atomicAdd(dimg + q * 4 + 1, acc.y); atomicAdd(dimg + q * 4 + 2, acc.z);
       }
     }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < KK * NK; i += blockDim.x) atomicAdd(dkern + static_cast<long long>(n) * KK * NK + i, sdk[i]);
+  // this block's dkern partial (warps summed in order) -> its own row of the scratch buffer dkern [gridDim.x][N][KK*NK]
+  for (int i = threadIdx.x; i < KK * NK; i += blockDim.x) {
+    float t = 0.f;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) t += sdk[w * KK * NK + i];
+    dkern[(static_cast<long long>(blockIdx.x) * N + n) * KK * NK + i] = t;
+  }
+}
+// dimage[q] += dT_NK[q] + sum_{taps, k} K[tap][k] * dT_k[p] over the pixels p whose reflected tap lands on q: a gather, so every
+// image gradient is summed in the same order on every run.  reflect_i(v) == q for v = q, -q - 1 and 2n - 1 - q.
+__global__ void __launch_bounds__(256) cdna_apply_bwd_dimage_kernel(const float* __restrict__ kern, const float* __restrict__ dA, int das,
+                                                                    const float* __restrict__ dB, int dbs, float* __restrict__ dimage, int N,
+                                                                    int H, int W, int KH, int KW, int NK) {
+  const int n = blockIdx.y;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= H * W) return;
+  const int qy = q / W, qx = q % W;
+  const int ph = (KH - 1) / 2, pw = (KW - 1) / 2;
+  const float* kn = kern + static_cast<long long>(n) * KH * KW * NK;
+  const long long base = static_cast<long long>(n) * H * W;
+  float3 acc;
+  {
+    const float4 a = *reinterpret_cast<const float4*>(dA + (base + q) * das + 4 * NK);
+    const float4 b = *reinterpret_cast<const float4*>(dB + (base + q) * dbs + 4 * NK);
+    acc = make_float3(a.x + b.x, a.y + b.y, a.z + b.z);
+  }
+  for (int i = 0; i < KH; ++i) {
+    const int vy[3] = {qy, -qy - 1, 2 * H - 1 - qy};
+    for (int cy = 0; cy < 3; ++cy) {
+      const int py = vy[cy] - i + ph;
+      if (py < 0 || py >= H) continue;
+      for (int j = 0; j < KW; ++j) {
+        const int vx[3] = {qx, -qx - 1, 2 * W - 1 - qx};
+        for (int cx = 0; cx < 3; ++cx) {
+          const int px = vx[cx] - j + pw;
+          if (px < 0 || px >= W) continue;
+          const long long o = base + static_cast<long long>(py) * W + px;
+          const float* kk = kn + (i * KW + j) * NK;
+          for (int k = 0; k < NK; ++k) {
+            const float4 a = *reinterpret_cast<const float4*>(dA + o * das + 4 * k);
+            const float4 b = *reinterpret_cast<const float4*>(dB + o * dbs + 4 * k);
+            acc.x += kk[k] * (a.x + b.x); acc.y += kk[k] * (a.y + b.y); acc.z += kk[k] * (a.z + b.z);
+          }
+        }
+      }
+    }
+  }
+  float* d = dimage + (base + q) * 4;
+  d[0] += acc.x; d[1] += acc.y; d[2] += acc.z;
 }
 
 // cdna kernel normalisation backward (see cdna_kernel_norm_kernel): raw/out/dout/draw [B][KK][NK]
@@ -569,7 +602,8 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ gates, const floa
 // ------------------------------------------------------------------------------------------------
 // reductions / elementwise
 // ------------------------------------------------------------------------------------------------
-// out[n][c] (+)= scale * sum_p x[n][p][c]   (bias gradients with n = 1; tile_concat / avg-pool adjoints)
+// part[blockIdx.y][n][c] = scale * sum_{p in the block's rows} x[n][p][c]; vp_colsum adds the parts to out in block order
+// (bias gradients with n = 1; tile_concat / avg-pool adjoints)
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, int xs, float* __restrict__ out, int os, int P,
                                                      int C, float scale, int rows_per_block) {
   const int n = blockIdx.z;
@@ -585,7 +619,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
   if (sub == 0 && c < C) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x & 31];
-    atomicAdd(out + static_cast<long long>(n) * os + c, t * scale);
+    out[(static_cast<long long>(blockIdx.y) * gridDim.z + n) * os + c] = t * scale;
   }
 }
 // dst[r][c] = (accumulate ? dst : 0) + scale[r / rows_per_scale or none] * src[r][c]
@@ -666,7 +700,7 @@ __global__ void __launch_bounds__(256) pixel_loss_kernel(const float* __restrict
     if (dpred) dpred[r * dps + c] = (mode & 2) ? dpred[r * dps + c] + g : g;   // bit 1: accumulate (l1 and l2 together)
   }
   bsum<1>(s, scratch);
-  if (threadIdx.x == 0) atomicAdd(out, s[0] * inv_count);
+  if (threadIdx.x == 0) out[blockIdx.x] = s[0] * inv_count;     // this block's part (scratch row), summed in block order
 }
 // losses.gan_loss for labels in {0, 1}: kind 0 = LSGAN mean (l - y)^2; kind 1 = GAN = mean sigmoid-cross-entropy(l, y);
 // kind 2 = SNGAN = mean softplus(l) (y = 0) / softplus(-l) (y = 1) -- numerically the same function as kind 1 for y in {0,1}.
@@ -739,7 +773,7 @@ __global__ void __launch_bounds__(256) cosine_distance_kernel(const float* __res
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i];
-    atomicAdd(out, t);
+    out[blockIdx.x] = t;                                          // this block's part (scratch row), summed in block order
   }
 }
 
@@ -792,7 +826,7 @@ __global__ void __launch_bounds__(256) cosine_distance_vec_kernel(const float* _
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i];
-    atomicAdd(out, t);
+    out[blockIdx.x] = t;                                          // this block's part (scratch row), summed in block order
   }
 }
 
@@ -842,10 +876,16 @@ extern "C" int vp_inorm_act_bwd(const float* x, int x_cstride, const float* cons
     cudaFuncSetAttribute(inorm_act_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4096 * 16);
     attr_set = true;
   }
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, 2LL * n * c, stream)) return -1;
   inorm_act_bwd_kernel<<<grid, positions >= 2048 ? 512 : 256, staged ? static_cast<size_t>(positions) * 32 : 0, as_stream(stream)>>>(
-      x, x_cstride, make_srcs(dy, dy_cstride, num_dy), dx, dx_cstride, positions, c, gamma, beta, stats, act, alpha, dgamma, dbeta,
-      staged);
-  return check_launch("inorm_act_bwd_kernel");
+      x, x_cstride, make_srcs(dy, dy_cstride, num_dy), dx, dx_cstride, positions, c, gamma, beta, stats, act, alpha, ws,
+      ws + static_cast<long long>(n) * c, staged);
+  int rc = check_launch("inorm_act_bwd_kernel");
+  if (!rc) rc = reduce_parts(ws, n, c, dgamma, stream);
+  if (!rc) rc = reduce_parts(ws + static_cast<long long>(n) * c, n, c, dbeta, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_lstm_gates_bwd(const float* pre, int n, int positions, int filters, const float* c_prev, const float* gamma1,
@@ -867,10 +907,19 @@ extern "C" int vp_lstm_gates_bwd(const float* pre, int n, int positions, int fil
     attr_set = true;
   }
   dim3 grid(filters / 4, n);
+  const long long nf = static_cast<long long>(n) * filters;
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, 10 * nf, stream)) return -1;
   lstm_gates_bwd_kernel<<<grid, positions >= 512 ? 512 : 256, smem, as_stream(stream)>>>(pre, positions, filters, c_prev, gamma1, beta1, gamma2, beta2,
                                                                stats1, stats2, forget_bias, make_srcs(dh, dh_cstride, num_dh),
-                                                               dc_next, dpre, dc_prev, dgamma1, dbeta1, dgamma2, dbeta2);
-  return check_launch("lstm_gates_bwd_kernel");
+                                                               dc_next, dpre, dc_prev, ws, ws + 4 * nf, ws + 8 * nf, ws + 9 * nf);
+  int rc = check_launch("lstm_gates_bwd_kernel");
+  if (!rc) rc = reduce_parts(ws, n, 4LL * filters, dgamma1, stream);
+  if (!rc) rc = reduce_parts(ws + 4 * nf, n, 4LL * filters, dbeta1, stream);
+  if (!rc) rc = reduce_parts(ws + 8 * nf, n, filters, dgamma2, stream);
+  if (!rc) rc = reduce_parts(ws + 9 * nf, n, filters, dbeta2, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_composite_bwd(const float* dgen, const float* masks, int masks_cstride, const float* layers, int layers_cstride,
@@ -886,10 +935,19 @@ extern "C" int vp_cdna_apply_bwd(const float* image, const float* kernels, const
                                  int d_b_cstride, float* dimage, float* dkernels, int n, int h, int w, int kh, int kw, int nk,
                                  vp_stream_t stream) {
   if (nk > 4) return set_error("vp_cdna_apply_bwd: at most 4 transformations");
+  if ((kh - 1) / 2 >= h || (kw - 1) / 2 >= w) return set_error("vp_cdna_apply_bwd: kernel larger than the image");
   dim3 grid((h * w + 255) / 256, n);
-  cdna_apply_bwd_kernel<<<grid, 256, 2 * kh * kw * nk * sizeof(float), as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(image), kernels, d_a, d_a_cstride, d_b, d_b_cstride, dimage, dkernels, n, h, w, kh, kw, nk);
-  return check_launch("cdna_apply_bwd_kernel");
+  const long long part = static_cast<long long>(n) * kh * kw * nk;
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, grid.x * part, stream)) return -1;
+  cdna_apply_bwd_kernel<<<grid, 256, 9 * kh * kw * nk * sizeof(float), as_stream(stream)>>>(
+      reinterpret_cast<const float4*>(image), kernels, d_a, d_a_cstride, d_b, d_b_cstride, dimage, ws, n, h, w, kh, kw, nk);
+  int rc = check_launch("cdna_apply_bwd_kernel");
+  if (!rc) rc = reduce_parts(ws, grid.x, part, dkernels, stream);
+  scratch_free(ws, stream);
+  if (rc) return rc;
+  cdna_apply_bwd_dimage_kernel<<<grid, 256, 0, as_stream(stream)>>>(kernels, d_a, d_a_cstride, d_b, d_b_cstride, dimage, n, h, w, kh, kw, nk);
+  return check_launch("cdna_apply_bwd_dimage_kernel");
 }
 
 extern "C" int vp_cdna_kernel_norm_bwd(const float* raw, const float* out, const float* dout, float* draw, int b, int kh, int kw,
@@ -940,8 +998,13 @@ extern "C" int vp_colsum(const float* x, int x_cstride, float* out, int out_stri
   const int rpb = 256;
   dim3 grid((c + 31) / 32, static_cast<unsigned>((positions + rpb - 1) / rpb), n);
   if (grid.y > 65535) return set_error("vp_colsum: too many rows");
-  colsum_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, x_cstride, out, out_stride, static_cast<int>(positions), c, scale, rpb);
-  return check_launch("colsum_kernel");
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, static_cast<long long>(grid.y) * n * c, stream)) return -1;
+  colsum_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, x_cstride, ws, c, static_cast<int>(positions), c, scale, rpb);
+  int rc = check_launch("colsum_kernel");
+  if (!rc) rc = reduce_parts_strided(ws, grid.y, n, c, out, out_stride, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_axpy_channels(const float* src, int src_cstride, float* dst, int dst_cstride, long long rows, int c, float scale,
@@ -978,9 +1041,14 @@ extern "C" int vp_pixel_loss(const float* pred, int pred_cstride, const float* t
                              float* out, vp_stream_t stream) {
   const float inv = 1.f / static_cast<float>(mean_count);
   const int blocks = static_cast<int>(std::min<long long>(1184, (rows * c + 255) / 256));
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, blocks, stream)) return -1;
   pixel_loss_kernel<<<blocks, 256, 0, as_stream(stream)>>>(pred, pred_cstride, target, target_cstride, dpred, dpred_cstride, rows, c,
-                                                           mode, inv, grad_scale, out);
-  return check_launch("pixel_loss_kernel");
+                                                           mode, inv, grad_scale, ws);
+  int rc = check_launch("pixel_loss_kernel");
+  if (!rc) rc = reduce_parts(ws, blocks, 1, out, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_gan_loss(const float* logits, float label, int n, float grad_scale, int kind, float* dlogits, float* out,
@@ -999,17 +1067,22 @@ extern "C" int vp_kl_loss(const float* mu, const float* lss, int rows, int nz, f
 extern "C" int vp_cosine_distance(const float* a, const float* b, float* da, long long rows, int c, float grad_scale, float* out,
                                   vp_stream_t stream) {
   const bool aligned = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(da)) & 15) == 0;
-  if (aligned && (c == 32 || c == 64 || c == 128)) {
-    const int lpr = c / 4;
-    const unsigned blocks = static_cast<unsigned>((rows * lpr + 255) / 256);
-    if (lpr == 8) cosine_distance_vec_kernel<8><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, out);
-    else if (lpr == 16) cosine_distance_vec_kernel<16><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, out);
-    else cosine_distance_vec_kernel<32><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, out);
-    return check_launch("cosine_distance_vec_kernel");
+  const bool vec = aligned && (c == 32 || c == 64 || c == 128);
+  const int lpr = c / 4;
+  const unsigned blocks = vec ? static_cast<unsigned>((rows * lpr + 255) / 256) : static_cast<unsigned>((rows + 7) / 8);
+  float* ws = nullptr;                                          // one loss part per block, summed in block order
+  if (scratch_alloc(&ws, blocks, stream)) return -1;
+  if (vec) {
+    if (lpr == 8) cosine_distance_vec_kernel<8><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, ws);
+    else if (lpr == 16) cosine_distance_vec_kernel<16><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, ws);
+    else cosine_distance_vec_kernel<32><<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, 1.f / rows, grad_scale, ws);
+  } else {
+    cosine_distance_kernel<<<blocks, 256, 0, as_stream(stream)>>>(a, b, da, rows, c, 1.f / rows, grad_scale, ws);
   }
-  cosine_distance_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, as_stream(stream)>>>(a, b, da, rows, c, 1.f / rows,
-                                                                                              grad_scale, out);
-  return check_launch("cosine_distance_kernel");
+  int rc = check_launch(vec ? "cosine_distance_vec_kernel" : "cosine_distance_kernel");
+  if (!rc) rc = reduce_parts(ws, blocks, 1, out, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_adam(float* p, const float* g, float* m, float* v, long long n, const float* lr_t, float beta1, float beta2,

@@ -1,26 +1,16 @@
 // Weight gradient of the FIRST video-discriminator layer (conv3d 3x3x3, stride 1, zero pad 1, <= 4 input channels
 // stored as float4 voxels, 32 output channels; networks.py:83-84) on the tensor cores.
 //
-//   gw[tap][ci][co] += sum_v x[v + tap][ci] * dy[v][co]            GEMM-K = voxels, M = (tap, ci), N = co
+//   gw[tap][ci][co] += sum_v x[v + tap][ci] * dy[v][co]            GEMM-K = voxels, M = (dx, ci), N = co
 //
-// With 4 input channels the generic wgrad engine wastes 7/8 of every 32-channel operand box, and the CUDA-core kernel it
-// replaces (conv3d_c4_wgrad_kernel, discrim.cu) is latency bound at ~0.9 ms per launch.  The only MN-major layout the
-// tensor core reads for 32-bit operands is the 128B swizzle with 32-byte atoms (tests/gpu_probe_umma.py: the un-swizzled
-// and 16-byte-atom layouts return zeros), whose fetch address is swizzle(start + (k%4)*128 + (k/4)*SBO + (m%32)*4 +
-// (m/32)*LBO), keyed on the absolute address, for any 32-byte-aligned start.  A line of float4 voxels IS such an operand:
-// the 32 M-elements of a 128-byte chunk are 8 consecutive voxels x 4 channels, and the chunk of K index k + 1 is the next
-// 8 voxels.  So with K = "every 8th voxel":
-//   * A(m = (g, j, ci), k) = halo_row[g][start + 8k + j][ci]: M-group g (LBO = row pitch) is one of four (dz, dy) halo rows,
-//     j a voxel offset 0..7 of which three are the taps dx = -1..1 (the other lanes are never stored), K walks the 64-voxel
-//     line segment in steps of 8.  A halo row is 10 voxel-octets from x0 - 8 (TMA box over a (32 floats = octet, W/8, H, D, N)
-//     view; borders are zero fill = the convolution's padding);
-//   * B(n = co, k) = dy[x0 + 8k + p][co] for phase p = 0..7: TMA delivers the dy tile phase-major ([p][k][co]) through a
-//     tensor map whose dimensions are (co, octet, phase, line) with strides (4 B, 1024 B, 128 B, W * 128 B);
-//   * phase p moves the A start by p voxels, but starts must be 32-byte aligned (a 16-byte start faults): even phases start
-//     at voxel p + 6 and find tap dx in lane group j = dx + 2, odd phases start at p + 7 and find it in j = dx + 1; the two
-//     parities accumulate in separate TMEM columns and are both added to gw by the epilogue.
-// Per 64 voxels: 10 TMA requests (9 rows + dy) issued by 10 lanes of one warp instruction, 24 MMAs of M = 128, N = 32
-// (8 phases x 3 groups of rows), accumulating in 2 x 96 TMEM columns over the CTA's whole voxel range.
+// With 4 input channels the generic wgrad engine wastes 7/8 of every 32-channel operand box, and the CUDA-core kernel
+// (conv3d_c4_wgrad_kernel, discrim.cu) is latency bound.  Here a line segment of 64 voxels is one pipeline stage: TMA
+// brings the 64 x 32 dy tile and the nine halo rows (dz, dy) of x, each 80 float4 voxels from x0 - 8 (borders are zero
+// fill = the convolution's padding).  For halo row r the three taps dx and the four channels are the 12 (of 16) M rows of
+// one m16n8k8 MMA whose A element (m = 4 dx + ci, k = v) is x_row[v + dx + 7][ci]: the overlapping voxels of the row are the
+// operand without any im2col.  Nine MMA warps (one per halo row) issue 4 x 8 MMAs per stage and keep their 16 x 32
+// accumulators in registers over the CTA's whole voxel range; each CTA stores its sum into its own scratch row, and the rows
+// are added to gw in CTA order (reduce_parts).
 #include <algorithm>
 #include <cstdint>
 #include <cstdlib>
@@ -31,41 +21,35 @@
 
 namespace vp {
 
-constexpr int kD0Pix = 64;                                   // voxels (GEMM-K x phases) per stage
+constexpr int kD0Pix = 64;                                   // voxels (GEMM-K) per stage
 constexpr int kD0RowOct = 10;                                // halo row box: voxels x0 - 8 .. x0 + 71
-constexpr int kD0RowBytes = kD0RowOct * 128;                 // = row pitch
+constexpr int kD0RowBytes = kD0RowOct * 128;
 constexpr int kD0DyBytes = kD0Pix * 128;
-constexpr int kD0StageBytes = 20 * 1024;                     // dy tile (8 KB, 1024-aligned) + 9 rows (11520 B)
+constexpr int kD0StageBytes = 20 * 1024;                     // dy tile (8 KB) + 9 rows (11520 B)
 constexpr int kD0Stages = 8;
-constexpr int kD0Tail = 8 * 1024;                            // the last row group's unused M-groups read past the last stage
+constexpr int kD0Threads = 320;                              // warp 0: TMA; warps 1..9: one halo row each
 
 struct D0WgradArgs {
   CUtensorMap xmap, dymap;
-  float* gw;
+  float* gw;                                                 // [gridDim.x][27 * CI * 32] per-CTA partial sums
   int tiles_w, H, D, N, CI;
   int total;                                                 // line segments = N * D * H * tiles_w
 };
 
-__global__ void __launch_bounds__(192, 1) d0_wgrad_kernel(const __grid_constant__ D0WgradArgs a) {
+__global__ void __launch_bounds__(kD0Threads, 1) d0_wgrad_kernel(const __grid_constant__ D0WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t full_bar[kD0Stages], empty_bar[kD0Stages], tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ uint64_t full_bar[kD0Stages], empty_bar[kD0Stages];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int it0 = static_cast<int>(static_cast<long long>(a.total) * blockIdx.x / gridDim.x);
   const int it1 = static_cast<int>(static_cast<long long>(a.total) * (blockIdx.x + 1) / gridDim.x);
   if (it1 <= it0) return;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kD0Stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(&tmem_full_bar, 1);
+    for (int i = 0; i < kD0Stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 9); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   const uint32_t smem0 = smem_u32(smem);
 
   if (warp == 0) {
@@ -88,7 +72,7 @@ __global__ void __launch_bounds__(192, 1) d0_wgrad_kernel(const __grid_constant_
       if (lane < 9) {
         tma_load_5d_addr(dst + kD0DyBytes + lane * kD0RowBytes, &a.xmap, fb, 0, tw * (kD0Pix / 8) - 1, y + ry, z + rz, n);
       } else if (lane == 9) {
-        tma_load_4d_addr(dst, &a.dymap, fb, 0, tw * (kD0Pix / 8), 0, line);
+        tma_load_2d_addr(dst, &a.dymap, fb, 0, line * (a.tiles_w * kD0Pix) + tw * kD0Pix);
       }
       if (++tw == a.tiles_w) {
         tw = 0; ++line;
@@ -96,81 +80,66 @@ __global__ void __launch_bounds__(192, 1) d0_wgrad_kernel(const __grid_constant_
       }
       if (++stage == kD0Stages) { stage = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      const uint32_t idesc = make_idesc_tf32(128, 32, 1, 1);
-      const uint64_t a_base = make_smem_desc(smem0 + kD0DyBytes, kD0RowBytes, 512, 0, 1);     // LBO: next halo row; SBO: 4 octets on
-      const uint64_t b_base = make_smem_desc(smem0, kD0DyBytes, 512, 0, 1);                    // one 32-channel group: LBO unused
-      uint32_t stage = 0, ph = 0, first = 1;
+    return;
+  }
+
+  const int r = warp - 1;                                      // halo row (dz, dy) = (r / 3, r % 3)
+  const int g = lane >> 2, t = lane & 3;
+  const int dx0 = g >> 2, ci = g & 3;                          // M row g = (dx0, ci); M row g + 8 = (dx0 + 2, ci)
+  float acc[4][4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+  uint32_t stage = 0, ph = 0;
 #pragma unroll 1
-      for (int it = it0; it < it1; ++it) {
-        mbar_wait(&full_bar[stage], ph);
-        tc_fence_after();
-        const uint32_t adv = stage * (kD0StageBytes >> 4);
+  for (int it = it0; it < it1; ++it) {
+    mbar_wait(&full_bar[stage], ph);
+    const uint32_t dyb = smem0 + stage * kD0StageBytes;
+    const uint32_t xr = dyb + kD0DyBytes + r * kD0RowBytes + static_cast<uint32_t>((dx0 + 7) * 4 + ci) * 4u;
 #pragma unroll
-        for (int p = 0; p < 8; ++p) {
-          // row voxel index of (k, p, dx) is 8k + p + dx + 8; the start must be even: p + 6 (even p) or p + 7 (odd p)
-          const uint32_t a_off = static_cast<uint32_t>((p & 1) ? p + 7 : p + 6);     // in 16-byte units
-          const uint32_t acc = (first && p < 2) ? 0u : 1u;
+    for (int k0 = 0; k0 < kD0Pix; k0 += 8) {
+      uint32_t af[4];
+      af[0] = lds_u32(xr + (k0 + t) * 16);
+      af[1] = lds_u32(xr + (k0 + t + 2) * 16);
+      af[2] = lds_u32(xr + (k0 + t + 4) * 16);
+      af[3] = lds_u32(xr + (k0 + t + 6) * 16);
 #pragma unroll
-          for (int rg = 0; rg < 3; ++rg)
-            umma_tf32(tmem_base + (p & 1) * 96 + rg * 32, a_base + adv + a_off + rg * (4 * kD0RowBytes >> 4), b_base + adv + p * (1024 >> 4),
-                      idesc, acc);
-        }
-        umma_commit(&empty_bar[stage]);
-        first = 0;
-        if (++stage == kD0Stages) { stage = 0; ph ^= 1; }
+      for (int j = 0; j < 4; ++j) {
+        uint32_t bf[2];
+        bf[0] = lds_u32(dyb + (k0 + t) * 128 + (8 * j + g) * 4);
+        bf[1] = lds_u32(dyb + (k0 + t + 4) * 128 + (8 * j + g) * 4);
+        mma_tf32_16x8x8(acc[j], af, bf);
       }
-      umma_commit(&tmem_full_bar);
     }
     __syncwarp();
-  } else {
-    // TMEM lane = 32 * g + 4 * j + ci: halo row 4 * rg + g, voxel offset j, input channel ci; the tap column is j - 1 in the
-    // even-phase accumulators (columns 0..95) and j in the odd-phase ones (columns 96..191)
-    const int g = warp & 3;
-    const int j = lane >> 2, ci = lane & 3;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int par = 0; par < 2; ++par) {
-      const int c = par ? j : j - 1;
-#pragma unroll 1
-      for (int rg = 0; rg < 3; ++rg) {
-        const int r = 4 * rg + g;
-        const bool valid = r < 9 && c >= 0 && c < 3 && ci < a.CI;
-        float* o = a.gw + (static_cast<long long>(r * 3 + c) * a.CI + ci) * 32;
-#pragma unroll 1
-        for (int cc = 0; cc < 32; cc += 16) {
-          float v[16];
-          __syncwarp();
-          tmem_ld16(tmem_base + (static_cast<uint32_t>(g * 32) << 16) + par * 96 + rg * 32 + cc, v);
-          if (valid) {
-#pragma unroll
-            for (int q = 0; q < 16; q += 4) red_add_v4(o + cc + q, v[q], v[q + 1], v[q + 2], v[q + 3]);
-          }
-        }
-      }
-    }
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == kD0Stages) { stage = 0; ph ^= 1; }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 256);
+  if (ci >= a.CI) return;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int dx = dx0 + 2 * h;
+    if (dx > 2) continue;
+    float* o = a.gw + static_cast<long long>(blockIdx.x) * 27 * a.CI * 32 + (static_cast<long long>(r * 3 + dx) * a.CI + ci) * 32 + 2 * t;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[j][2 * h], acc[j][2 * h + 1]);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // FORWARD of the same layer: out[v][co] = lrelu(bias[co] + sum_{dz,dy,dx,ci} x[v + (dz,dy,dx)][ci] * w[dz][dy][dx][ci][co] / sigma).
 //
-// GEMM M = voxels, N = 32, K = (tap, ci).  The un-swizzled K-major UMMA layout has core matrices of 8 rows x 16 bytes
+// GEMM M = voxels, N = 32, K = (tap, ci).  The un-swizzled K-major wgmma layout has core matrices of 8 rows x 16 bytes
 // stored as 128 contiguous bytes, i.e. eight consecutive float4 voxels are eight A rows whose first four K elements are the
 // voxel's channels; the next four K elements sit LBO bytes further, and LBO = 16 makes them the NEXT voxel (tap dx + 1):
 // the overlapping rows x[v-1 .. v+2] are the K = 16 operand of one kernel row (the dx = +2 column meets zero weights) without
 // any im2col.  To give 128 consecutive A rows a uniform 16-byte pitch the halo tile is kept FLAT: TMA writes (L + 2) lines
 // of (W + 2) voxels back to back, a 128-row M tile is 128 consecutive flat positions (about two lines) and the two halo
 // positions per line produce outputs that are not stored (3 %).  The generic engine needed 27 taps x 32 padded channels
-// (8x the MMAs, 270 us per 32 clips); this kernel issues 18 MMAs per 128 voxels.
+// (8x the MMAs); this kernel issues 18 MMAs (K = 8) per 64 voxels and warpgroup.
 // Work item = (sample, frame, block of L lines): three TMA boxes (the planes z-1, z, z+1), double buffered; weights / sigma,
-// TF32-rounded, are laid out once per CTA as the B operand; accumulators rotate through four 32-column TMEM buffers.
-constexpr int kF0Acc = 4;
+// TF32-rounded, are laid out once per CTA as the B operand.  Warpgroup 0 loads, warpgroups 1 and 2 each own one 64-row half
+// of every 128-row tile and apply bias + leaky relu from their accumulator registers.
+constexpr int kF0Threads = 384;
 
 struct D0FwdArgs {
   CUtensorMap xmap;
@@ -183,13 +152,12 @@ struct D0FwdArgs {
   int pitch, plane_bytes, plane_stride, stage_bytes, tiles, items, hblocks;   // plane_stride: plane_bytes rounded to the 128 B TMA alignment
 };
 
-__global__ void __launch_bounds__(192, 1) d0_fwd_kernel(const __grid_constant__ D0FwdArgs a) {
+__global__ void __launch_bounds__(kF0Threads, 1) d0_fwd_kernel(const __grid_constant__ D0FwdArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t full_bar[2], empty_bar[2], acc_full[kF0Acc], acc_empty[kF0Acc];
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ __align__(16) float stage[4][32][36];                  // epilogue transpose tiles (one per epilogue warp)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ uint64_t full_bar[2], empty_bar[2];
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
   constexpr int kWBytes = 18 * 1024;                                  // B operand: [row 9][k-step 2][32 n x 8 k = 1 KB]
   if (static_cast<int>(blockIdx.x) >= a.items) return;
 
@@ -213,122 +181,93 @@ __global__ void __launch_bounds__(192, 1) d0_fwd_kernel(const __grid_constant__ 
     fence_proxy_async();
   }
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < kF0Acc; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   const uint32_t smem0 = smem_u32(smem);
   const uint32_t stage0 = smem0 + kWBytes;
 
-  if (warp == 0) {
-    uint32_t stage = 0, ph = 0;
-#pragma unroll 1
-    for (int item = blockIdx.x; item < a.items; item += gridDim.x) {
-      int t = item;
-      const int hb = t % a.hblocks; t /= a.hblocks;
-      const int z = t % a.D;
-      const int n = t / a.D;
-      mbar_wait(&empty_bar[stage], ph ^ 1);
-      if (lane == 0) mbar_expect_tx(&full_bar[stage], 3u * static_cast<uint32_t>(a.plane_bytes));
-      __syncwarp();
-      if (lane < 3)
-        tma_load_5d_addr(stage0 + stage * a.stage_bytes + lane * a.plane_stride, &a.xmap, smem_u32(&full_bar[stage]), 0, -1, hb * a.L - 1,
-                         z + lane - 1, n);
-      if (++stage == 2) { stage = 0; ph ^= 1; }
-    }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      const uint32_t idesc = make_idesc_tf32(128, 32, 0, 0);
-      const uint64_t a_base = make_smem_desc(stage0, 16, 128, 0, 0);      // LBO 16 B: K elements 4..7 = the next voxel; SBO: 8 voxels
-      const uint64_t b_base = make_smem_desc(smem0, 128, 256, 0, 0);
-      uint32_t stage = 0, ph = 0, tcount = 0;
+  if (wg == 0) {
+    if (threadIdx.x < 32) {
+      uint32_t stage = 0, ph = 0;
 #pragma unroll 1
       for (int item = blockIdx.x; item < a.items; item += gridDim.x) {
-        mbar_wait(&full_bar[stage], ph);
-        tc_fence_after();
-        const uint32_t sadv = stage * (static_cast<uint32_t>(a.stage_bytes) >> 4);
-#pragma unroll 1
-        for (int tile = 0; tile < a.tiles; ++tile, ++tcount) {
-          const uint32_t acc = tcount % kF0Acc;
-          mbar_wait(&acc_empty[acc], ((tcount / kF0Acc) & 1) ^ 1);
-          tc_fence_after();
-          // A row m of this tile = flat position p0 + m; tap (dz, dy, dx) reads flat voxel p + (dy + 1) * pitch + dx + 1 of plane dz + 1
-          const uint32_t p0 = sadv + static_cast<uint32_t>(tile) * 128u;          // in 16-byte units = voxels
-#pragma unroll
-          for (int r = 0; r < 9; ++r) {
-            const uint32_t row_off = static_cast<uint32_t>(r / 3) * (static_cast<uint32_t>(a.plane_stride) >> 4) +
-                                     static_cast<uint32_t>(r % 3) * static_cast<uint32_t>(a.pitch);
-#pragma unroll
-            for (int s = 0; s < 2; ++s)
-              umma_tf32(tmem_base + acc * 32, a_base + p0 + row_off + 2 * s, b_base + (r * 2 + s) * (1024 >> 4), idesc, (r | s) ? 1u : 0u);
-          }
-          umma_commit(&acc_full[acc]);
-        }
-        umma_commit(&empty_bar[stage]);
+        int t = item;
+        const int hb = t % a.hblocks; t /= a.hblocks;
+        const int z = t % a.D;
+        const int n = t / a.D;
+        mbar_wait(&empty_bar[stage], ph ^ 1);
+        if (lane == 0) mbar_expect_tx(&full_bar[stage], 3u * static_cast<uint32_t>(a.plane_bytes));
+        __syncwarp();
+        if (lane < 3)
+          tma_load_5d_addr(stage0 + stage * a.stage_bytes + lane * a.plane_stride, &a.xmap, smem_u32(&full_bar[stage]), 0, -1, hb * a.L - 1,
+                           z + lane - 1, n);
         if (++stage == 2) { stage = 0; ph ^= 1; }
       }
     }
-    __syncwarp();
-  } else {
-    const int q = warp & 3;
-    float bv[32];
+    return;
+  }
+
+  const int h = wg - 1, wq = (threadIdx.x >> 5) & 3;
+  const uint64_t a_base = make_wgmma_desc(stage0 + h * 64 * 16, 16, 128, kWgmmaInterleave);   // LBO 16 B: K elements 4..7 = the next voxel; SBO: 8 voxels
+  const uint64_t b_base = make_wgmma_desc(smem0, 128, 256, kWgmmaInterleave);
+  float bv[8];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) bv[j] = a.bias ? __ldg(a.bias + j) : 0.f;
-    uint32_t tcount = 0;
+  for (int i = 0; i < 4; ++i) {
+    const int co = 8 * i + 2 * (lane & 3);
+    bv[2 * i] = a.bias ? __ldg(a.bias + co) : 0.f;
+    bv[2 * i + 1] = a.bias ? __ldg(a.bias + co + 1) : 0.f;
+  }
+  uint32_t stage = 0, ph = 0;
+  float acc[16];
 #pragma unroll 1
-    for (int item = blockIdx.x; item < a.items; item += gridDim.x) {
-      int t = item;
-      const int hb = t % a.hblocks; t /= a.hblocks;
-      const int z = t % a.D;
-      const int n = t / a.D;
-      float* obase = a.out + ((static_cast<long long>(n) * a.D + z) * a.H + static_cast<long long>(hb) * a.L) * a.W * 32;
+  for (int item = blockIdx.x; item < a.items; item += gridDim.x) {
+    int t = item;
+    const int hb = t % a.hblocks; t /= a.hblocks;
+    const int z = t % a.D;
+    const int n = t / a.D;
+    float* obase = a.out + ((static_cast<long long>(n) * a.D + z) * a.H + static_cast<long long>(hb) * a.L) * a.W * 32;
+    mbar_wait(&full_bar[stage], ph);
+    const uint32_t sadv = stage * (static_cast<uint32_t>(a.stage_bytes) >> 4);
 #pragma unroll 1
-      for (int tile = 0; tile < a.tiles; ++tile, ++tcount) {
-        const uint32_t acc = tcount % kF0Acc;
-        mbar_wait(&acc_full[acc], (tcount / kF0Acc) & 1);
-        tc_fence_after();
-        float v[32];
-        __syncwarp();
-        tmem_ld16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 32, v);
-        tmem_ld16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 32 + 16, v + 16);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[acc]);
-        // bias + leaky relu, then through a per-warp shared tile so that every store instruction writes 512 contiguous bytes
-        // (a lane owns one voxel = 128 B; storing straight from the registers touches 32 different lines per instruction)
-        float (*st)[36] = stage[q];
+    for (int tile = 0; tile < a.tiles; ++tile) {
+      // A row m of this tile = flat position p0 + m; tap (dz, dy, dx) reads flat voxel p + (dy + 1) * pitch + dx + 1 of plane dz + 1
+      const uint32_t p0 = sadv + static_cast<uint32_t>(tile) * 128u;          // in 16-byte units = voxels
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float r4[4];
+      for (int r = 0; r < 9; ++r) {
+        const uint32_t row_off = static_cast<uint32_t>(r / 3) * (static_cast<uint32_t>(a.plane_stride) >> 4) +
+                                 static_cast<uint32_t>(r % 3) * static_cast<uint32_t>(a.pitch);
 #pragma unroll
-          for (int c = 0; c < 4; ++c) { const float u = v[j + c] + bv[j + c]; r4[c] = fmaxf(u, a.alpha * u); }
-          *reinterpret_cast<float4*>(&st[lane][j]) = make_float4(r4[0], r4[1], r4[2], r4[3]);
+        for (int s = 0; s < 2; ++s)
+          Wgmma<32>::mma(acc, a_base + p0 + row_off + 2 * s, b_base + (r * 2 + s) * (1024 >> 4), (r | s) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int p = tile * 128 + 64 * h + 16 * wq + (lane >> 2) + 8 * rr;
+        const int line = p / a.pitch, i = p - line * a.pitch;
+        if (line < a.L && i < a.W) {
+          float* o = obase + (static_cast<long long>(line) * a.W + i) * 32 + 2 * (lane & 3);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const float u0 = acc[4 * q + 2 * rr] + bv[2 * q], u1 = acc[4 * q + 2 * rr + 1] + bv[2 * q + 1];
+            *reinterpret_cast<float2*>(o + 8 * q) = make_float2(fmaxf(u0, a.alpha * u0), fmaxf(u1, a.alpha * u1));
+          }
         }
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int row = j * 4 + (lane >> 3), quad = lane & 7;
-          const int p = tile * 128 + q * 32 + row;
-          const int line = p / a.pitch, i = p - line * a.pitch;
-          if (line < a.L && i < a.W)
-            *reinterpret_cast<float4*>(obase + (static_cast<long long>(line) * a.W + i) * 32 + quad * 4) = *reinterpret_cast<const float4*>(&st[row][quad * 4]);
-        }
-        __syncwarp();
       }
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == 2) { stage = 0; ph ^= 1; }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 128);
 }
 
 static int encode_map(CUtensorMap* m, const float* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
-                      CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) {
+                      CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_NONE) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return set_error("cuTensorMapEncodeTiled entry point not found");
   cuuint32_t es[5] = {1, 1, 1, 1, 1};
@@ -352,37 +291,37 @@ extern "C" int vp_conv3d_c4_wgrad_tc(const float* x, const float* dy, float* gw,
   if (total <= 0 || total > 0x7fffffffLL) return set_error("vp_conv3d_c4_wgrad_tc: bad dims");
   D0WgradArgs A;
   {
-    // x: (octet of float4 voxels, w / 8, h, d, n), halo row boxes of 10 octets; dy: (channel, octet, phase, line) so that a 64-voxel box arrives
-    // phase-major: [phase][octet][32 channels]
+    // x: (octet of float4 voxels, w / 8, h, d, n), halo row boxes of 10 octets; dy: (channel, voxel of all lines), 64-voxel boxes
     const cuuint64_t W = wd, H = h, Dd = d;
     cuuint64_t xd[5] = {32, W / 8, H, Dd, static_cast<cuuint64_t>(n)};
     cuuint64_t xs[4] = {128, 16 * W, 16 * W * H, 16 * W * H * Dd};
     cuuint32_t xb[5] = {32, kD0RowOct, 1, 1, 1};
     if (encode_map(&A.xmap, x, 5, xd, xs, xb)) return -1;
-    cuuint64_t yd[4] = {32, W / 8, 8, static_cast<cuuint64_t>(n) * Dd * H};
-    cuuint64_t ys[3] = {1024, 128, 128 * W};
-    cuuint32_t yb[4] = {32, 8, 8, 1};
-    if (encode_map(&A.dymap, dy, 4, yd, ys, yb)) return -1;
+    cuuint64_t yd[2] = {32, static_cast<cuuint64_t>(n) * Dd * H * W};
+    cuuint64_t ys[1] = {128};
+    cuuint32_t yb[2] = {32, kD0Pix};
+    if (encode_map(&A.dymap, dy, 2, yd, ys, yb)) return -1;
   }
-  A.gw = gw;
   A.tiles_w = wd / kD0Pix; A.H = h; A.D = d; A.N = n; A.CI = ci;
   A.total = static_cast<int>(total);
-  const size_t smem = static_cast<size_t>(kD0Stages) * kD0StageBytes + kD0Tail + 1024;
+  const size_t smem = static_cast<size_t>(kD0Stages) * kD0StageBytes + 1024;
   static bool configured = false;
   if (!configured) {
     if (cudaFuncSetAttribute(d0_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) != cudaSuccess)
       return set_error("cudaFuncSetAttribute(d0_wgrad_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
     configured = true;
   }
-  int sms = 148;
-  {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
+  const int sms = device_sms();
   const int grid = static_cast<int>(std::min<long long>(sms, total));
-  d0_wgrad_kernel<<<grid, 192, smem, as_stream(stream)>>>(A);
-  return check_launch("d0_wgrad_kernel");
+  const long long part = 27LL * ci * 32;
+  float* ws = nullptr;
+  if (scratch_zeroed(&ws, grid * part, stream)) return -1;     // a CTA with no line segment leaves its row zero
+  A.gw = ws;
+  d0_wgrad_kernel<<<grid, kD0Threads, smem, as_stream(stream)>>>(A);
+  int rc = check_launch("d0_wgrad_kernel");
+  if (!rc) rc = reduce_parts(ws, grid, part, gw, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_conv3d_c4_fwd_tc(const float* x, const float* w, const float* inv_scale, const float* bias, float* out, int n, int d, int h,
@@ -426,13 +365,8 @@ extern "C" int vp_conv3d_c4_fwd_tc(const float* x, const float* w, const float* 
       return set_error("cudaFuncSetAttribute(d0_fwd_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
     configured = smem;
   }
-  int sms = 148;
-  {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
+  const int sms = device_sms();
   const int grid = static_cast<int>(std::min<long long>(sms, items));
-  d0_fwd_kernel<<<grid, 192, smem, as_stream(stream)>>>(A);
+  d0_fwd_kernel<<<grid, kF0Threads, smem, as_stream(stream)>>>(A);
   return check_launch("d0_fwd_kernel");
 }

@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(256) sn_rowdot_kernel(const float* __restrict_
   s = wsum2(s);
   if (lane == 0) out[r] = s;
 }
-// out[c] += sum_r vec[r] * W[r][c]   (rows split over blockIdx.y; out zero-filled by caller)
+// part[blockIdx.y][c] = sum_{r in the block's rows} vec[r] * W[r][c]   (rows split over blockIdx.y; summed in block order)
 __global__ void __launch_bounds__(256) sn_coldot_kernel(const float* __restrict__ W, const float* __restrict__ vec,
                                                         float* __restrict__ out, int R, int C, int rows_per_block) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31), sub = threadIdx.x >> 5;
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(256) sn_coldot_kernel(const float* __restrict_
   if (sub == 0 && c < C) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x & 31];
-    atomicAdd(out + c, t);
+    out[static_cast<long long>(blockIdx.y) * C + c] = t;
   }
 }
 // v = t/(|t|+eps) in place; scal[0] = |t|
@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(1024) sn_finish_kernel(const float* __restrict
   for (int i = threadIdx.x; i < n; i += blockDim.x) u_new[i] = s[i] * inv;
   if (threadIdx.x == 0) { scal[1] = nrm; scal[2] = q * inv; }
 }
-// scal[3] += <G, W>
+// part[blockIdx.x] = this block's share of <G, W>
 __global__ void __launch_bounds__(256) sn_dot_kernel(const float* __restrict__ G, const float* __restrict__ W, long long n,
                                                      float* __restrict__ scal) {
   __shared__ float scratch[32];
@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(256) sn_dot_kernel(const float* __restrict__ G
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     s += G[i] * W[i];
   s = block_reduce(s, scratch);
-  if (threadIdx.x == 0) atomicAdd(scal + 3, s);
+  if (threadIdx.x == 0) scal[blockIdx.x] = s;
 }
 // gs[c] = a * s_hat[c] * gsigma, gsigma = -<G,W>/sigma^2, a = (|s|^2+2 eps |s|)/(|s|+eps)^2, s_hat = s/|s|
 __global__ void sn_bwd_gs_kernel(const float* __restrict__ s, float* __restrict__ gs, int n, const float* __restrict__ scal) {
@@ -152,7 +152,14 @@ extern "C" int vp_spectral_norm_fwd(const float* w, const float* u, int rows, in
   cudaMemsetAsync(s, 0, sizeof(float) * cols, st);
   const int rpb = 512;
   dim3 grid((cols + 31) / 32, (rows + rpb - 1) / rpb);
-  sn_coldot_kernel<<<grid, 256, 0, st>>>(w, v, s, rows, cols, rpb);                   // s = v W
+  {
+    float* ws = nullptr;
+    if (scratch_alloc(&ws, static_cast<long long>(grid.y) * cols, stream)) return -1;
+    sn_coldot_kernel<<<grid, 256, 0, st>>>(w, v, ws, rows, cols, rpb);                  // s = v W, block partials
+    const int rc = reduce_parts(ws, grid.y, cols, s, stream);
+    scratch_free(ws, stream);
+    if (rc) return rc;
+  }
   sn_finish_kernel<<<1, 1024, 0, st>>>(s, u_new, cols, scal);                         // u' = l2n(s), sigma
   count_launch(3);
   return check_launch("spectral_norm_fwd");
@@ -163,7 +170,15 @@ extern "C" int vp_spectral_norm_bwd(const float* w, const float* u, const float*
   cudaStream_t st = as_stream(stream);
   const long long n = static_cast<long long>(rows) * cols;
   cudaMemsetAsync(scal + 3, 0, sizeof(float), st);
-  sn_dot_kernel<<<static_cast<int>(std::min<long long>(592, (n + 255) / 256)), 256, 0, st>>>(g_wbar, w, n, scal);
+  {
+    const int blocks = static_cast<int>(std::min<long long>(592, (n + 255) / 256));
+    float* ws = nullptr;
+    if (scratch_alloc(&ws, blocks, stream)) return -1;
+    sn_dot_kernel<<<blocks, 256, 0, st>>>(g_wbar, w, n, ws);
+    const int rc = reduce_parts(ws, blocks, 1, scal + 3, stream);
+    scratch_free(ws, stream);
+    if (rc) return rc;
+  }
   sn_bwd_gs_kernel<<<(cols + 127) / 128, 128, 0, st>>>(s, gs, cols, scal);
   sn_rowdot_kernel<<<(rows + 7) / 8, 256, 0, st>>>(w, gs, gt, rows, cols);            // gv = W gs
   sn_bwd_gt_kernel<<<1, 1024, 0, st>>>(v, gt, rows, scal);
@@ -318,7 +333,7 @@ extern "C" int vp_conv3d_c4_wgrad(const float* x, const float* dy, float* gw, in
   if (ci < 1 || ci > 3) return set_error("vp_conv3d_c4_wgrad: 1..3 input channels");
   const long long total = static_cast<long long>(n) * d * h * wd;
   // ~3 resident blocks per SM per temporal tap: each warp walks one contiguous chunk of voxels
-  const long long target_warps = 148LL * 3 * 8;
+  const long long target_warps = 24LL * device_sms();
   const int chunk = static_cast<int>(std::max<long long>(64, (total + target_warps - 1) / target_warps));
   const long long warps = (total + chunk - 1) / chunk;
   dim3 grid(static_cast<unsigned>((warps + 7) / 8), 3);

@@ -275,8 +275,9 @@ __global__ void __launch_bounds__(256) dense_fwd_kernel(const float* __restrict_
       for (int w2 = 0; w2 < nw; ++w2) t += red[w2][warp][lane];
       t *= sc;
       if (bias && blockIdx.y == 0) t += bias[j];
-      float* o = y + static_cast<long long>(b0 + warp) * ys + j;
-      if (gridDim.y > 1) atomicAdd(o, t); else *o = t;
+      // with K split over blockIdx.y, y is a scratch buffer of dense [B][J] parts (ys = J), summed in block order by the host
+      float* o = y + static_cast<long long>(blockIdx.y) * B * ys + static_cast<long long>(b0 + warp) * ys + j;
+      *o = t;
     }
     __syncthreads();
   }
@@ -341,7 +342,7 @@ __global__ void __launch_bounds__(256) dense_fwd_tiled_kernel(const float* __res
         if (j >= J) continue;
         float v = acc[r][c] * sc;
         if (bias && blockIdx.x == 0) v += bias[j];
-        atomicAdd(y + static_cast<long long>(b) * ys + j, v);
+        y[(static_cast<long long>(blockIdx.x) * B + b) * ys + j] = v;      // this block's part of a K-split sum (dense rows)
       }
     }
   }
@@ -555,14 +556,30 @@ extern "C" int vp_dense_fwd(const float* x, int x_stride, const float* w, const 
   // wide layers called with k_splits > 1 (y zero-filled by the caller): tiled kernel
   const size_t tsm = (64 * static_cast<size_t>((j + 3) & ~3) + 64 * static_cast<size_t>((b + 3) & ~3)) * sizeof(float);
   if (k_splits > 1 && k >= 1024 && j <= 128 && tsm <= 48 * 1024) {
-    dense_fwd_tiled_kernel<<<(k + 63) / 64, 256, tsm, as_stream(stream)>>>(x, x_stride, w, bias, inv_scale, y, y_stride, b, k, j);
-    return check_launch("dense_fwd_tiled_kernel");
+    // the K blocks write their parts into scratch rows, which are added to y in block order (run-to-run identical sums)
+    const int parts = (k + 63) / 64;
+    float* ws = nullptr;
+    if (scratch_zeroed(&ws, static_cast<long long>(parts) * b * j, stream)) return -1;
+    dense_fwd_tiled_kernel<<<parts, 256, tsm, as_stream(stream)>>>(x, x_stride, w, bias, inv_scale, ws, j, b, k, j);
+    int rc = check_launch("dense_fwd_tiled_kernel");
+    if (!rc) rc = reduce_parts_strided(ws, parts, b, j, y, y_stride, stream);
+    scratch_free(ws, stream);
+    return rc;
   }
   if (k_splits < 1) k_splits = 1;
   const int kchunk = (k + k_splits - 1) / k_splits;
   dim3 grid((b + 3) / 4, (k + kchunk - 1) / kchunk);
-  dense_fwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, x_stride, w, bias, inv_scale, y, y_stride, b, k, j, kchunk);
-  return check_launch("dense_fwd_kernel");
+  if (grid.y == 1) {
+    dense_fwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, x_stride, w, bias, inv_scale, y, y_stride, b, k, j, kchunk);
+    return check_launch("dense_fwd_kernel");
+  }
+  float* ws = nullptr;
+  if (scratch_zeroed(&ws, static_cast<long long>(grid.y) * b * j, stream)) return -1;
+  dense_fwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, x_stride, w, bias, inv_scale, ws, j, b, k, j, kchunk);
+  int rc = check_launch("dense_fwd_kernel");
+  if (!rc) rc = reduce_parts_strided(ws, grid.y, b, j, y, y_stride, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 extern "C" int vp_lstm_cell_fwd(const float* gates, const float* c_prev, float* c_new, float* h_new, int b, int units,

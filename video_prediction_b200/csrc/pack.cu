@@ -5,7 +5,7 @@
 //   PLAIN      Keff = w
 //   POOLED     conv_pool2d (ops.py:838-842): the 2x2 average pool is applied to the kernel
 //   UPSAMPLED  upsample_conv2d (ops.py:698-704): bilinear 4x4 (x) kernel, FULL correlation
-// and stored K-major, zero padded and rounded to TF32 (round-to-nearest), in the layout the UMMA
+// and stored K-major, zero padded and rounded to TF32 (round-to-nearest), in the layout the wgmma
 // descriptors read:  FWD  [tap][co -> n_pad][ci -> kc*32],  DGRAD [tap][ci -> n_pad][co -> kc*32].
 // A channel map lets the engine's internal (16-byte aligned, padded) concat layouts differ from the
 // reference's channel order.
@@ -191,7 +191,7 @@ extern "C" int vp_tf32_residual(const float* x, float* lo, long long n, vp_strea
   if (!x || !lo || (n & 3) || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(lo) & 15))
     return set_error("vp_tf32_residual: pointers must be 16B aligned and n a multiple of 4");
   const long long n4 = n / 4;
-  const int blocks = static_cast<int>(std::min<long long>(148 * 8, (n4 + 255) / 256));
+  const int blocks = static_cast<int>(std::min<long long>(8LL * device_sms(), (n4 + 255) / 256));
   tf32_residual_kernel<<<std::max(blocks, 1), 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(x),
                                                                           reinterpret_cast<float4*>(lo), n4);
   return check_launch("tf32_residual_kernel");

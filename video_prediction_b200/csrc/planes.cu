@@ -189,8 +189,8 @@ __global__ void __launch_bounds__(512) slab_inorm_act_bwd_kernel(const float* __
   if (blockIdx.x == 0 && pl == 0) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      atomicAdd(dbeta + c0 + i, s[i]);
-      atomicAdd(dgamma + c0 + i, s[4 + i]);
+      dbeta[static_cast<long long>(n) * C + c0 + i] = s[i];
+      dgamma[static_cast<long long>(n) * C + c0 + i] = s[4 + i];
     }
   }
   const float inv = 1.f / P;
@@ -251,8 +251,8 @@ __global__ void __launch_bounds__(512) slab_inorm_act_bwd_loop_kernel(const floa
   if (blockIdx.x == 0 && pl == 0) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      atomicAdd(dbeta + c0 + i, s[i]);
-      atomicAdd(dgamma + c0 + i, s[4 + i]);
+      dbeta[static_cast<long long>(n) * C + c0 + i] = s[i];
+      dgamma[static_cast<long long>(n) * C + c0 + i] = s[4 + i];
     }
   }
   const float inv = 1.f / P;
@@ -473,8 +473,8 @@ __global__ void __launch_bounds__(512) slab_gates_bwd_kernel(
   if (blockIdx.x == 0 && pl == 0) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      atomicAdd(db2 + c0 + k, sA[k]);
-      atomicAdd(dg2 + c0 + k, sA[4 + k]);
+      db2[static_cast<long long>(n) * F + c0 + k] = sA[k];
+      dg2[static_cast<long long>(n) * F + c0 + k] = sA[4 + k];
     }
   }
   // ---- pass B: dc' -> gate gradients (w.r.t. the normalised + affine gates); sums for the gate norm
@@ -533,8 +533,8 @@ __global__ void __launch_bounds__(512) slab_gates_bwd_kernel(
     for (int g = 0; g < 4; ++g)
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        atomicAdd(db1 + g * F + c0 + k, sB[4 * g + k]);
-        atomicAdd(dg1 + g * F + c0 + k, sB[16 + 4 * g + k]);
+        db1[static_cast<long long>(n) * 4 * F + g * F + c0 + k] = sB[4 * g + k];
+        dg1[static_cast<long long>(n) * 4 * F + g * F + c0 + k] = sB[16 + 4 * g + k];
       }
   }
   // ---- pass C: gate-norm backward -> dpre
@@ -570,9 +570,8 @@ static bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 // cluster size cs (1..8), positions per CTA ppc = P / cs, and for the register-resident kernels lanes * iters = ppc.
 //
 // The candidates are ranked by how many ROUNDS of resident clusters the launch needs: these kernels hold one CTA per SM
-// (registers or 160-200 KB of staging), and a cluster of 8 is placed inside a GPC, so only 15 clusters of 8 (120 CTAs) are
-// co-resident on the 148 SMs -- the first version launched 32 clusters of 8 for the 32x32 planes and ran three rounds of a
-// latency-bound kernel (ncu: launch__cluster_max_active 15, SMs active 53 % of the time).  cudaOccupancyMaxActiveClusters
+// (registers or 160-200 KB of staging), and a cluster of 8 is placed inside a GPC, so fewer CTAs than SMs are co-resident
+// in clusters of 8; launching more clusters than fit runs extra rounds of a latency-bound kernel.  cudaOccupancyMaxActiveClusters
 // gives the resident cluster count of each candidate; cost = rounds * (1 + ppc / ppc_ref): a round is a fixed latency chain
 // (loads, two cluster-wide reductions, stores) plus a part that grows with the positions a CTA walks.
 struct SlabPlan { int cs, ppc, lanes, iters; };
@@ -598,7 +597,7 @@ static int max_active_clusters(const void* kernel, int cs, int threads, size_t s
   int n = 0;
   if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess || n < 1) {
     cudaGetLastError();
-    n = std::max(1, 148 / cs);
+    n = std::max(1, device_sms() / cs);
   }
   cache[key] = n;
   return n;
@@ -704,11 +703,21 @@ int slab_inorm_act_bwd(const float* x, int xs, const float* const* dy, const int
   for (int i = 0; i < 4; ++i) { s.ptr[i] = i < num_dy ? dy[i] : nullptr; s.stride[i] = i < num_dy ? dy_cs[i] : 0; }
   dim3 grid(pl.cs, C / 32, n);
   K k = pick(pl.iters);
+  // per-sample partials of dgamma / dbeta (rows of the scratch buffer), added to the outputs in sample order
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, 2LL * n * C, stream)) return -1;
+  float *wg = ws, *wb = ws + static_cast<long long>(n) * C;
+  int rc;
   if (!k)
-    return launch_cluster(slab_inorm_act_bwd_loop_kernel, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta,
-                          stats, act, alpha, dgamma, dbeta, pl.cs, pl.ppc);
-  return launch_cluster(k, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta, stats, act, alpha, dgamma,
-                        dbeta, pl.cs);
+    rc = launch_cluster(slab_inorm_act_bwd_loop_kernel, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta,
+                        stats, act, alpha, wg, wb, pl.cs, pl.ppc);
+  else
+    rc = launch_cluster(k, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta, stats, act, alpha, wg, wb,
+                        pl.cs);
+  if (rc == 0) rc = reduce_parts(wg, n, C, dgamma, stream);
+  if (rc == 0) rc = reduce_parts(wb, n, C, dbeta, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 int slab_gates_fwd(const float* pre, int n, int P, int F, const float* c_prev, const float* g1, const float* b1, const float* g2,
@@ -768,8 +777,19 @@ int slab_gates_bwd(const float* pre, int n, int P, int F, const float* c_prev, c
   s.count = num_dh;
   for (int i = 0; i < 4; ++i) { s.ptr[i] = i < num_dh ? dh[i] : nullptr; s.stride[i] = i < num_dh ? dh_cs[i] : 0; }
   dim3 grid(pl.cs, F / 32, n);
-  return launch_cluster(slab_gates_bwd_kernel, grid, pl.lanes * 8, staging(pl.ppc), pl.cs, as_stream(stream), pre, P, F, c_prev, g1, b1, g2, b2,
-                        stats1, stats2, forget_bias, s, dc_next, dpre, dc_prev, dg1, db1, dg2, db2, pl.cs, pl.ppc);
+  // per-sample partials of the four norm-parameter gradients, added to the outputs in sample order
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, 10LL * n * F, stream)) return -1;
+  const long long nf = static_cast<long long>(n) * F;
+  float *w_dg1 = ws, *w_db1 = ws + 4 * nf, *w_dg2 = ws + 8 * nf, *w_db2 = ws + 9 * nf;
+  int rc = launch_cluster(slab_gates_bwd_kernel, grid, pl.lanes * 8, staging(pl.ppc), pl.cs, as_stream(stream), pre, P, F, c_prev, g1, b1, g2, b2,
+                          stats1, stats2, forget_bias, s, dc_next, dpre, dc_prev, w_dg1, w_db1, w_dg2, w_db2, pl.cs, pl.ppc);
+  if (rc == 0) rc = reduce_parts(w_dg1, n, 4LL * F, dg1, stream);
+  if (rc == 0) rc = reduce_parts(w_db1, n, 4LL * F, db1, stream);
+  if (rc == 0) rc = reduce_parts(w_dg2, n, F, dg2, stream);
+  if (rc == 0) rc = reduce_parts(w_db2, n, F, db2, stream);
+  scratch_free(ws, stream);
+  return rc;
 }
 
 }  // namespace vp

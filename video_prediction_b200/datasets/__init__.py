@@ -1,6 +1,6 @@
 """Dataset registry with the reference's surface (video_prediction/datasets/__init__.py:11-25).
 
-The TFRecord input pipelines sit either side of the B200 hot path (SURVEY.md 8f-3).  The two formats the BASELINE configs
+The TFRecord input pipelines sit either side of the H100 hot path (SURVEY.md 8f-3).  The two formats the BASELINE configs
 train on are read on the host without TensorFlow (`video_datasets.py`, `tfrecord.py`): BAIR robot pushing (`softmotion` /
 `bair`) and KTH (`kth`); the other registered names (JPEG-encoded or unused by any shipped config) raise
 NotImplementedError.  `synthetic` is the dataset the hot path is measured on:

@@ -80,7 +80,6 @@ def geom(k, s=(1, 1, 1), p=(0, 0, 0), transposed=False):
     return VpConvGeom(k[0], k[1], k[2], s[0], s[1], s[2], p[0], p[1], p[2], int(transposed))
 
 
-_ENGINE_CHOICE = {}     # geometry signature -> 0 (box) / 1 (halo), measured once per process
 _PROFILE = None         # list of (kind, algorithmic flops, start event, end event) while profile_engine(True) is active
 
 
@@ -148,80 +147,23 @@ def _conv_key(x_view, g, n_pad, kc, out_view, act, extra):
             out_view.c == out_view.cstride, g.kd, g.kh, g.kw, g.sd, g.sh, g.sw, g.pd, g.ph, g.pw, g.transposed, n_pad, kc, act, extra)
 
 
-def _pick_engine(key, call, idempotent, out_view=None):
-    """Both engines compute the same convolution; which one is faster depends on the geometry (plane size, taps per halo
-    group, N).  The first call of a geometry times both (CUDA-graph replays) and the winner is cached for the process.
-    VP_HALO=0/1 or VP_AUTOTUNE=0 pin the engine.  A call that accumulates into its output is timed on a snapshot: the output
-    tensor is cloned before and restored after (possible when the view was made by tensor_view), otherwise it is not timed."""
-    choice = _ENGINE_CHOICE.get(key)
-    if choice is not None:
-        return choice
-    owner = getattr(out_view, '_owner', None)
-    if os.environ.get('VP_AUTOTUNE', '1') == '0' or 'VP_HALO' in os.environ or torch.cuda.is_current_stream_capturing() or \
-            (not idempotent and owner is None):
-        return -1
-    snapshot = owner.clone() if not idempotent else None
-    times = []
-    for eng in (0, 1):
-        check(lib().vp_conv_set_engine(eng))
-        call()                                   # warm-up (function attributes, descriptor cache)
-        torch.cuda.synchronize()
-        # the kernels are shorter than an eager launch costs on the host (ctypes + tensor-map encoding), so 8 launches are
-        # captured into a CUDA graph and the replay is timed: GPU time, not launch rate
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for _ in range(8):
-                call()
-        g.replay()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        g.replay()
-        g.replay()
-        e1.record()
-        e1.synchronize()
-        times.append(e0.elapsed_time(e1) * 3.0 / 16.0)      # keeps the unit of the log: milliseconds per 3 launches
-        del g
-    check(lib().vp_conv_set_engine(-1))
-    if snapshot is not None:
-        owner.copy_(snapshot)
-    choice = 0 if times[0] <= times[1] else 1
-    _ENGINE_CHOICE[key] = choice
-    if os.environ.get('VP_AUTOTUNE_LOG'):
-        import sys
-        sys.stderr.write('[autotune] %s box %.1f us halo %.1f us -> %s\n' % (key, times[0] / 3 * 1e3, times[1] / 3 * 1e3, 'halo' if choice else 'box'))
-    return choice
-
-
 def conv_igemm(x_view, g, wpacked, n_pad, kc, out_view, bias=None, act=ACT_NONE, alpha=0.0, split_k=1, accumulate=0):
     if 'igemm' in _SKIP:
         return
-
-    def call():
-        check(lib().vp_conv_igemm(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view), ptr(bias),
-                                  act, C.c_float(alpha), split_k, int(accumulate), stream_ptr()))
-    # an explicit split_k > 1 adds atomically into a caller-cleared output: repeating the call (timing) would change it
     key = _conv_key(x_view, g, n_pad, kc, out_view, act, ('fwd', split_k))
-    eng = _pick_engine(key, call, not accumulate and split_k <= 1, out_view if split_k <= 1 else None)
-    check(lib().vp_conv_set_engine(eng))
-    _profiled('igemm', _conv_flops(x_view, g, out_view), call, (key, eng))
-    if eng >= 0:
-        check(lib().vp_conv_set_engine(-1))
+    _profiled('igemm', _conv_flops(x_view, g, out_view),
+              lambda: check(lib().vp_conv_igemm(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view), ptr(bias),
+                                                act, C.c_float(alpha), split_k, int(accumulate), stream_ptr())), key)
 
 
 def conv_igemm_actgrad(x_view, g, wpacked, n_pad, kc, out_view, act_output_addr, addend_addr, act, alpha=0.0, accumulate=0):
     if 'igemm' in _SKIP:
         return
-
-    def call():
-        check(lib().vp_conv_igemm_actgrad(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view),
-                                          C.c_void_p(act_output_addr), C.c_void_p(addend_addr or 0), act, C.c_float(alpha),
-                                          int(accumulate), stream_ptr()))
     key = _conv_key(x_view, g, n_pad, kc, out_view, act, ('actgrad', bool(addend_addr)))
-    eng = _pick_engine(key, call, not accumulate, out_view)
-    check(lib().vp_conv_set_engine(eng))
-    _profiled('igemm', _conv_flops(x_view, g, out_view), call, (key, eng))
-    if eng >= 0:
-        check(lib().vp_conv_set_engine(-1))
+    _profiled('igemm', _conv_flops(x_view, g, out_view),
+              lambda: check(lib().vp_conv_igemm_actgrad(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view),
+                                                        C.c_void_p(act_output_addr), C.c_void_p(addend_addr or 0), act,
+                                                        C.c_float(alpha), int(accumulate), stream_ptr())), key)
 
 
 def tf32_residual(x):
@@ -245,7 +187,7 @@ def conv_wgrad(x_view, dy_view, g, dwpacked, n_pad, kc, split_k=1):
     flops = 2.0 * dy_view.n * dy_view.d * dy_view.h * dy_view.w * dy_view.c * x_view.c * taps
     _profiled('wgrad', flops, lambda: check(lib().vp_conv_wgrad(C.byref(x_view), C.byref(dy_view), C.byref(g), ptr(dwpacked), n_pad, kc,
                                                                split_k, stream_ptr())),
-              (_conv_key(x_view, g, n_pad, kc, dy_view, 0, ('wgrad', split_k)), -1))
+              _conv_key(x_view, g, n_pad, kc, dy_view, 0, ('wgrad', split_k)))
 
 
 def eff_taps(k, kind):

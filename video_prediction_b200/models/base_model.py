@@ -3,7 +3,7 @@
 Keeps the constructor signature, hparams defaults/override order, mode / context_frames /
 sequence_length validation (base_model.py:20-59), the learning-rate and KL-weight schedules
 (:286-319) and the `build_graph(inputs)` entry point (:467).  There is no TF graph: build_graph
-allocates device buffers and the compute is the sm_100a kernels in libvp_b200.so."""
+allocates device buffers and the compute is the sm_90a kernels in libvp_b200.so."""
 from __future__ import annotations
 
 import itertools

@@ -1,4 +1,4 @@
-"""SAVP model on B200: host-side orchestration of the sm_100a kernels in libvp_b200.so.
+"""SAVP model on H100: host-side orchestration of the sm_90a kernels in libvp_b200.so.
 
 Mirrors `SAVPVideoPredictionModel` of the reference (video_prediction/models/savp_model.py:771-855):
 same constructor, same default hparams (:779-822), same deprecated-key handling (:824-846), same
@@ -9,7 +9,7 @@ unroll out in HBM as time-stacked channels-last buffers ([T-1, NB, H, W, C']) wh
 *is* the concatenation each convolution reads (image | first image | z), (features | z | h_prev),
 (features | skip | z): producers write straight into their consumers' slices, `tile_concat` is a
 broadcast store, and the posterior and prior unrolls (savp_model.py:730-732, shared weights) run as
-one batch NB = 2B.  All FLOP-carrying ops are tcgen05 implicit GEMMs (csrc/igemm.cu); the rest are
+one batch NB = 2B.  All FLOP-carrying ops are tensor-core implicit GEMMs (csrc/igemm.cu); the rest are
 HBM-bound kernels (csrc/elementwise.cu).  PyTorch only owns memory and streams.
 """
 from __future__ import annotations
@@ -235,7 +235,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             if hp.kl_weight and hp.kl_anneal not in ('none', 'sigmoid', 'linear'):
                 unsupported.append('kl_anneal=%r' % (hp.kl_anneal,))
         if unsupported:
-            raise NotImplementedError('hparams outside the B200 hot path (SURVEY.md 8f): ' + ', '.join(unsupported))
+            raise NotImplementedError('hparams outside the H100 hot path (SURVEY.md 8f): ' + ', '.join(unsupported))
 
     # ------------------------------------------------------------------ structure (savp_model.py:182-232)
     @staticmethod
@@ -347,7 +347,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         `set_params` was called, and all activation buffers."""
         super(SAVPVideoPredictionModel, self).build_graph(inputs)
         if not torch.cuda.is_available():
-            raise RuntimeError('video_prediction_b200 needs a CUDA device (sm_100a); there is no CPU fallback')
+            raise RuntimeError('video_prediction_b200 needs a CUDA device (sm_90a); there is no CPU fallback')
         L.lib()  # fail loudly if the CUDA library is missing
         self._check_supported()
         hp = self.hparams
@@ -391,9 +391,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if self.world_size > 1:     # replicas start from rank 0's variables (post_init_ops, base_model.py:640-646)
             dp.broadcast_state([self.g_flat, self.d_flat] + [v for k, v in self.params.items() if k.endswith('/u')])
         self._allreduce = dp.make_allreduce()
-        # VP_DP_BUCKETS=1: per-tower / per-layer all-reduces overlapped with the backward pass (dp.GradientReducer).  Measured at
-        # 2 GPUs: 34.37 ms/step with buckets, 34.25 without (33.89 on one GPU) -- 18 extra NCCL launches cost what the overlap
-        # saves when two ~100 us all-reduces are all there is to hide, so the default stays two flat all-reduces
+        # VP_DP_BUCKETS=1: per-tower / per-layer all-reduces overlapped with the backward pass (dp.GradientReducer); the default
+        # is two flat all-reduces (one per optimizer), which cost the fewest NCCL launches
         self._reducer = dp.GradientReducer(self.device) if (self.world_size > 1 and os.environ.get('VP_DP_BUCKETS', '0') == '1') else None
         self._build_generator()
         if self.mode == 'train':

@@ -1,10 +1,10 @@
-"""Training half of the SAVP path on B200: spectrally-normalised video discriminators, losses,
+"""Training half of the SAVP path on H100: spectrally-normalised video discriminators, losses,
 back-propagation through time over the time-stacked buffers, and the two TF-style Adam steps.
 
 Restates the reference's single-tower training graph (base_model.py:402-516): per step
   UPDATE_OPS(u) -> D forward on {enc_real, enc_fake, real, fake} -> d_loss -> D grads -> Adam(D)
   -> D forward again with the updated weights (new clip offsets) -> g_loss_post -> G grads -> Adam(G).
-All convolution gradients run on the tcgen05 engine: dgrad = the same implicit GEMM with the
+All convolution gradients run on the tensor-core engine: dgrad = the same implicit GEMM with the
 transposed-flag flipped and [ci][co] tap matrices; wgrad = one MN-major GEMM per layer over ALL
 timesteps of the unroll at once (GEMM-K = (T-1)*NB*H*W pixels) instead of per-step accumulation."""
 from __future__ import annotations
@@ -97,16 +97,16 @@ class SNLayer(object):
     @property
     def cuda_core(self):
         """First layer (3 colour channels -> 32): runs on the CUDA-core kernels of csrc/discrim.cu.  With 4 channels per
-        tap the tensor-core engine issues one K = 8 MMA per 24 KB pipeline stage and is ring-latency bound: measured
-        44.0 ms/step against 40.2 ms/step with these kernels (VP_D0_CUDA_CORE=0 selects the engine for comparison)."""
+        tap the generic tensor-core engine would pad every operand to 32 channels and issue one K = 8 MMA per pipeline stage
+        (VP_D0_CUDA_CORE=0 selects the engine for comparison)."""
         if os.environ.get('VP_D0_CUDA_CORE', '1') != '1':
             return False
         return (not self.is_fc) and not self.two_d and self.k == 3 and tuple(self.stride) == (1, 1, 1) and self.cin_ref <= 3 and self.co == 32
 
     def fwd(self, x, out):
-        # the first layer has its own tensor-core kernels (csrc/d0_layer.cu): float4 voxel rows are UMMA operands as they lie
+        # the first layer has its own tensor-core kernels (csrc/d0_layer.cu): float4 voxel rows are tensor-core operands as they lie
         # -- forward: overlapping rows x[v-1 .. v+2] = the K = 16 operand of a kernel row, 18 MMAs per 128 voxels against
-        # 108 on the generic engine (270 us -> ~40 us per 32 clips); weight gradient: ~80 us against 900 us on the CUDA cores.
+        # 108 on the generic engine; weight gradient: the overlapping voxels of a halo row as the (dx, ci) x voxel operand.
         # The fp32-exact mode runs the generic engine (3xTF32) and the exact CUDA-core weight gradient.
         if self.cuda_core and not L.exact_mode():
             P = self.m.params

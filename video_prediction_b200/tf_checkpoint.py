@@ -1,6 +1,6 @@
 """Reader for TensorFlow checkpoints ("tensor bundle", V2: `<prefix>.index` + `<prefix>.data-00000-of-0000N`) without
 TensorFlow -- SURVEY.md 8f-1: lets the pretrained SAVP weights the reference distributes
-(pretrained_models/download_model.sh) drive the B200 path through `model.restore()`.
+(pretrained_models/download_model.sh) drive the H100 path through `model.restore()`.
 
 Formats restated from TensorFlow's published sources (tensorflow/core/util/tensor_bundle/tensor_bundle.{h,cc},
 tensorflow/core/lib/io/table*.cc, tensorflow/core/protobuf/tensor_bundle.proto, tensor_shape.proto):

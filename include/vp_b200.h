@@ -61,7 +61,8 @@ int vp_version(void);
  * split_k > 1: partial sums are atomically added into `out` (caller zero-fills; act must be NONE;
  * bias is added by split 0), so the fp32 result depends on the order the splits finish in.  split_k == 0 and 1: unsplit
  * (run-to-run identical results).  accumulate = 1: out += result (act must be NONE);
- * accumulate = 2: out = act(out + result + bias) -- the last pass of a multi-pass (3xTF32) accumulation. */
+ * accumulate = 2: out = act(out + result + bias) -- the last pass of a multi-pass (3xTF32) accumulation; needs
+ * split_k <= 1.  Any other accumulate value is an error. */
 int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
                   const vp_tensor* out, const float* bias, int act, float alpha, int split_k, int accumulate,
                   vp_stream_t stream);
@@ -80,7 +81,9 @@ int vp_tf32_residual(const float* x, float* lo, long long n, vp_stream_t stream)
 
 /* Weight gradient of the same convolution: dwpacked[tap][co][ci] += sum_o  dy.. * x..
  * (layout VP_WLAYOUT_FWD: rows = channels of dy (n_pad rows), cols = kc*32 channels of x).
- * Always accumulates atomically: caller zero-fills before the first call of a step. */
+ * Accumulates into dwpacked without atomics: each element has one owner per pixel-range split, and several splits are
+ * added in split order from zero-filled scratch (run-to-run identical results).  The caller zero-fills dwpacked before
+ * the first call of a step. */
 int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked, int n_pad,
                   int kc, int split_k, vp_stream_t stream);
 

@@ -330,10 +330,10 @@ def test_full_length_generator_matches_oracle(Model, name, hk, B, shape, A):
 # ---------------------------------------------------------------------------------------------- graph replay vs eager
 def test_captured_step_reproduces_the_eager_step(Model, tmp_path):
     """The step bench.py times is ONE captured CUDA graph with parallel branches (discriminator towers, spectral norm + packing
-    under the generator forward).  From the same checkpoint and batch: the eager step, a captured replay and a second replay
-    must produce the same losses and gradients up to what summation-order noise becomes in TF32 arithmetic (atomics in split-K
-    and the weight gradients reorder fp32 sums; downstream truncations to TF32 flip).  A step
-    that is not executed at capture time (the bug this test found), a stale buffer or a race between branches shows as O(1)."""
+    under the generator forward).  From the same checkpoint and batch, the eager step, a captured replay and a second replay
+    must produce bit-identical losses and gradients: every sum that many blocks contribute to in this configuration is reduced
+    in a fixed order (DESIGN.md, run-to-run reproducibility), so any difference is a race, a stale buffer, a step that is not
+    executed at capture time, or a float atomic that came back."""
     import make_golden_b16 as G
     hp, params, inputs, noise = G.case()
     binp = {'images': inputs['images'].permute(1, 0, 2, 3, 4)}
@@ -355,11 +355,12 @@ def test_captured_step_reproduces_the_eager_step(Model, tmp_path):
             runs.append((model.g_grad.clone(), model.d_grad.clone(), model.loss_vals.clone()))
         grads[how] = runs
 
-    def rel(a, b):
-        return ((a - b).double().norm() / b.double().norm()).item()
+    def differs(a, b):
+        return (a != b).sum().item()
     (g0, d0, l0), (g1, d1, l1) = grads['graph']
     ge, de, le = grads['eager'][0]
-    errs = dict(replay_vs_replay=(rel(g0, g1), rel(d0, d1), rel(l0, l1)), graph_vs_eager=(rel(g0, ge), rel(d0, de), rel(l0, le)))
-    print('captured-step reproducibility (relative L2 of the flat G / D gradients, loss vector):', errs)
-    assert max(errs['replay_vs_replay'][:2]) < 5e-3 and errs['replay_vs_replay'][2] < 1e-3, errs
-    assert max(errs['graph_vs_eager'][:2]) < 3e-2 and errs['graph_vs_eager'][2] < 1e-3, errs
+    errs = dict(replay_vs_replay=(differs(g0, g1), differs(d0, d1), differs(l0, l1)),
+                graph_vs_eager=(differs(g0, ge), differs(d0, de), differs(l0, le)))
+    print('captured-step reproducibility (differing elements of the flat G / D gradients and the loss vector):', errs)
+    assert torch.equal(g0, g1) and torch.equal(d0, d1) and torch.equal(l0, l1), errs
+    assert torch.equal(g0, ge) and torch.equal(d0, de) and torch.equal(l0, le), errs

@@ -502,6 +502,10 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
   if (in->n != out->n) return set_error("vp_conv_igemm: batch mismatch");
   if (split_k > 1 && act != VP_ACT_NONE) return set_error("vp_conv_igemm: split_k needs act NONE");
   if (aux_y && split_k > 1) return set_error("vp_conv_igemm: the fused activation gradient needs split_k <= 1");
+  if (accumulate < 0 || accumulate > 2) return set_error("vp_conv_igemm: accumulate must be 0, 1 or 2 (got %d)", accumulate);
+  // every split would read the existing partial sum and add it again, as many times as there are splits
+  if (accumulate == 2 && split_k > 1)
+    return set_error("vp_conv_igemm: accumulate = 2 needs split_k <= 1 (got split_k = %d)", split_k);
   static thread_local IgemmArgs A;  // large POD; per-thread host-side scratch (ctypes releases the GIL during calls)
   std::memset(&A, 0, sizeof(A));
   const int lat[4] = {out->w, out->h, out->d, out->n};

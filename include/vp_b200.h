@@ -255,13 +255,12 @@ int vp_spectral_norm_fwd(const float* w, const float* u, int rows, int cols, flo
                          float* scal, vp_stream_t stream);
 int vp_spectral_norm_bwd(const float* w, const float* u, const float* g_wbar, int rows, int cols, const float* v,
                          const float* s, float* scal, float* gs, float* gt, float* dw, vp_stream_t stream);
-/* First discriminator layer on the CUDA cores (conv3d 3x3x3, stride 1, zero pad 1, <= 4 input channels stored as
- * float4 voxels, 32 output channels, fused bias + leaky relu; networks.py:83-84).  w is the REFERENCE-layout kernel
- * [3][3][3][ci][32]; it is divided by *inv_scale (spectral-norm sigma).  wgrad accumulates dL/d(w/sigma) into gw. */
-int vp_conv3d_c4_fwd(const float* x, const float* w, const float* inv_scale, const float* bias, float* out, int n, int d,
-                     int h, int wd, int ci, float lrelu_alpha, vp_stream_t stream);
+/* First discriminator layer (conv3d 3x3x3, stride 1, zero pad 1, <= 4 input channels stored as float4 voxels, 32 output
+ * channels; networks.py:83-84).  Weight gradient on the CUDA cores in exact fp32 (1..3 input channels, any width):
+ * accumulates dL/d(w/sigma) into gw [3][3][3][ci][32]. */
 int vp_conv3d_c4_wgrad(const float* x, const float* dy, float* gw, int n, int d, int h, int wd, int ci, vp_stream_t stream);
-/* The same layer on the tensor cores (TF32 operands, fp32 accumulate), without repacking x (csrc/d0_layer.cu):
+/* The same layer on the tensor cores (TF32 operands, fp32 accumulate), without repacking x (csrc/d0_layer.cu).  fwd: fused
+ * bias + leaky relu; w is the REFERENCE-layout kernel [3][3][3][ci][32], divided by *inv_scale (spectral-norm sigma).
  *  fwd:   a flat halo tile of float4 voxels is the un-swizzled K-major wgmma operand; the next-voxel leading offset
  *         (LBO = 16 B) turns x[v-1 .. v+2] into the K = 16 operand of one kernel row.  Needs h % 4 == 0 and a tile that fits
  *         (64^2, 128^2 do).

@@ -317,18 +317,15 @@ def test_cosine_distance_vectorised_shapes(L, rows, C):
     close(da - 0.25, torch.autograd.grad(3.0 * ref, ad)[0], 1e-6, 'cosine distance grad')
 
 
-def test_conv3d_c4_cuda_core_first_discriminator_layer(L):
+def test_conv3d_c4_wgrad_cuda_cores(L):
+    """vp_conv3d_c4_wgrad (the exact CUDA-core weight gradient of the first discriminator layer) against fp64 autograd."""
     N, D, H, W, C = 2, 5, 16, 12, 3
     x = torch.zeros(N, D, H, W, 4, device='cuda')
     x[..., :C] = torch.rand(N, D, H, W, C, device='cuda')
     w, b, dy = rnd(3, 3, 3, C, 32, seed=1, scale=0.2), rnd(32, seed=2), rnd(N, D, H, W, 32, seed=3)
-    sigma = torch.tensor([1.7], device='cuda')
-    out = torch.zeros(N, D, H, W, 32, device='cuda')
-    L.conv3d_c4_fwd(x, w, sigma, b, out, N, D, H, W, C, 0.1)
     wb = (w.double() / 1.7).requires_grad_(True)
     xp = F.pad(x[..., :C].double(), (0, 0, 1, 1, 1, 1, 1, 1))
     pre = O.conv3d_tf_valid(xp, wb, (1, 1, 1), b.double())
-    close(out, O.lrelu(pre, 0.1), 1e-5, 'conv3d_c4 fwd')
     (gw,) = torch.autograd.grad(pre, wb, dy.double())
     g = torch.zeros(27 * C * 32, device='cuda')
     L.conv3d_c4_wgrad(x, dy, g, N, D, H, W, C)
@@ -361,9 +358,9 @@ def test_conv3d_c4_wgrad_tensor_cores(L, N, D, H, W, C):
 
 
 @pytest.mark.parametrize('N,D,H,W,C', [(2, 3, 16, 64, 3), (1, 2, 8, 128, 1), (3, 4, 64, 64, 3), (1, 2, 12, 20, 2)])
-def test_conv3d_c4_fwd_tensor_cores(L, N, D, H, W, C):
+def test_conv3d_c4_fwd_tensor_cores_vs_fp64(L, N, D, H, W, C):
     """vp_conv3d_c4_fwd_tc (flat halo tile of float4 voxels as the un-swizzled K-major operand, LBO = one voxel) against the
-    fp64 convolution of the operands the tensor core sees (x truncated to TF32, w / sigma rounded to TF32) and the CUDA-core kernel."""
+    fp64 convolution of the operands the tensor core sees (x truncated to TF32, w / sigma rounded to TF32)."""
     def trunc(t):
         return (t.contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32)
     x = torch.zeros(N, D, H, W, 4, device='cuda')
@@ -376,9 +373,6 @@ def test_conv3d_c4_fwd_tensor_cores(L, N, D, H, W, C):
     xp = F.pad(trunc(x)[..., :C].double(), (0, 0, 1, 1, 1, 1, 1, 1))
     ref = O.lrelu(O.conv3d_tf_valid(xp, tf32(w / sigma).double(), (1, 1, 1), b.double()), 0.1)
     close(out, ref, 2e-5, 'first layer forward on the tensor cores')
-    out2 = torch.zeros_like(out)
-    L.conv3d_c4_fwd(x, w, sigma, b, out2, N, D, H, W, C, 0.1)
-    close(out, out2, 3e-3, 'tensor cores vs CUDA cores')
 
 
 def test_pack_weights_batch_equals_per_tensor_packs(L):
@@ -392,7 +386,7 @@ def test_pack_weights_batch_equals_per_tensor_packs(L):
         cmap = torch.arange(ci_int, dtype=torch.int32, device='cuda')
         cmap[ci:] = -1
         sigma = torch.tensor([1.3 + i], device='cuda') if i % 2 else None
-        for layout in (L.WLAYOUT_FWD, L.WLAYOUT_DGRAD):
+        for layout in (L.WLAYOUT_FWD, L.WLAYOUT_DGRAD, L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL, L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL):
             ref, n_pad, kc = L.pack_weights(w, k, ci, co, kind, layout, ci_int=ci_int, cmap=cmap, inv_scale=sigma)
             out = torch.full_like(ref, -7.0)
             entries.append((w, k, ci, co, kind, layout, ci_int, cmap, sigma, out))

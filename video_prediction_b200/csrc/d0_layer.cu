@@ -337,7 +337,7 @@ extern "C" int vp_conv3d_c4_fwd_tc(const float* x, const float* w, const float* 
   for (int cand : {16, 8, 4}) {
     if (h % cand == 0 && 3LL * (cand + 2) * A.pitch * 16 <= 90 * 1024) { L = cand; break; }
   }
-  if (!L || A.pitch > 256) return set_error("vp_conv3d_c4_fwd_tc: %d x %d frames do not tile (use vp_conv3d_c4_fwd)", h, wd);
+  if (!L || A.pitch > 256) return set_error("vp_conv3d_c4_fwd_tc: %d x %d frames do not tile", h, wd);
   A.L = L;
   A.plane_bytes = (L + 2) * A.pitch * 16;
   A.plane_stride = (A.plane_bytes + 127) / 128 * 128;

@@ -206,60 +206,12 @@ extern "C" int vp_scatter_clip(const float* dclip, const int32_t* t_start, float
 }
 
 // ------------------------------------------------------------------------------------------------
-// First discriminator layer (networks.py:83-84: conv3d 3x3x3, stride 1, zero pad 1, C_in = colour channels <= 4,
-// C_out = ndf = 32).  With 3 input channels the implicit GEMM wastes > 95 % of every tensor-core tile, and the layer is
-// bandwidth-sized anyway (168 MB of output per 32 clips), so it runs on the CUDA cores:
-//   forward : thread = (voxel, 8 output channels); a warp shares the 8-channel group -> weight reads are broadcasts
-//   wgrad   : lane = output channel; a warp walks a chunk of voxels keeping the 27*C_in partial sums in registers
+// Weight gradient of the first discriminator layer (networks.py:83-84: conv3d 3x3x3, stride 1, zero pad 1, C_in = colour
+// channels <= 3, C_out = ndf = 32) on the CUDA cores, in exact fp32: the fp32-exact mode's kernel, and the fallback for
+// widths the tensor-core kernel (d0_layer.cu) does not tile.  lane = output channel; a warp walks a chunk of voxels keeping
+// the 27*C_in partial sums in registers.
 // ------------------------------------------------------------------------------------------------
 namespace vp {
-
-__global__ void __launch_bounds__(256) conv3d_c4_fwd_kernel(const float4* __restrict__ x, const float* __restrict__ w,
-                                                            const float* __restrict__ inv_scale, const float* __restrict__ bias,
-                                                            float* __restrict__ out, int N, int D, int H, int W, int CI,
-                                                            float alpha) {
-  __shared__ float sw[27 * 4 * 32];
-  const float sc = inv_scale ? 1.f / __ldg(inv_scale) : 1.f;
-  for (int i = threadIdx.x; i < 27 * 4 * 32; i += blockDim.x) {
-    const int co = i & 31, ci = (i >> 5) & 3, t = i >> 7;
-    sw[i] = ci < CI ? w[(t * CI + ci) * 32 + co] * sc : 0.f;
-  }
-  __syncthreads();
-  const int cg = threadIdx.x >> 6;                    // 4 groups of 8 output channels; uniform per warp
-  const long long v = static_cast<long long>(blockIdx.x) * 64 + (threadIdx.x & 63);
-  const long long total = static_cast<long long>(N) * D * H * W;
-  if (v >= total) return;
-  const int xw = static_cast<int>(v % W);
-  const int yh = static_cast<int>((v / W) % H);
-  const int zd = static_cast<int>((v / (static_cast<long long>(W) * H)) % D);
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = bias ? bias[cg * 8 + j] : 0.f;
-#pragma unroll
-  for (int dz = -1; dz <= 1; ++dz) {
-    const bool zin = static_cast<unsigned>(zd + dz) < static_cast<unsigned>(D);
-#pragma unroll
-    for (int dy = -1; dy <= 1; ++dy) {
-      const bool yin = static_cast<unsigned>(yh + dy) < static_cast<unsigned>(H);
-#pragma unroll
-      for (int dx = -1; dx <= 1; ++dx) {
-        const bool in = zin && yin && static_cast<unsigned>(xw + dx) < static_cast<unsigned>(W);
-        const float4 xv = in ? x[v + (static_cast<long long>(dz) * H + dy) * W + dx] : make_float4(0.f, 0.f, 0.f, 0.f);
-        const int t = (dz + 1) * 9 + (dy + 1) * 3 + (dx + 1);
-        const float* wt = sw + t * 128 + cg * 8;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          acc[j] += xv.x * wt[j] + xv.y * wt[32 + j] + xv.z * wt[64 + j] + xv.w * wt[96 + j];
-      }
-    }
-  }
-  float4* o = reinterpret_cast<float4*>(out + v * 32 + cg * 8);
-  float r[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) r[j] = fmaxf(alpha * acc[j], acc[j]);
-  o[0] = make_float4(r[0], r[1], r[2], r[3]);
-  o[1] = make_float4(r[4], r[5], r[6], r[7]);
-}
 
 // gw[(t*CI + ci)*32 + co] += sum_v x[v + tap_t][ci] * dy[v][co]
 // blockIdx.y selects the temporal tap dz (9 of the 27 taps -> 27 accumulators per lane, high occupancy); lane = output
@@ -318,15 +270,6 @@ __global__ void __launch_bounds__(256, 3) conv3d_c4_wgrad_kernel(const float4* _
 }
 
 }  // namespace vp
-
-extern "C" int vp_conv3d_c4_fwd(const float* x, const float* w, const float* inv_scale, const float* bias, float* out, int n,
-                                int d, int h, int wd, int ci, float lrelu_alpha, vp_stream_t stream) {
-  if (ci < 1 || ci > 4) return set_error("vp_conv3d_c4_fwd: 1..4 input channels");
-  const long long total = static_cast<long long>(n) * d * h * wd;
-  conv3d_c4_fwd_kernel<<<static_cast<unsigned>((total + 63) / 64), 256, 0, as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(x), w, inv_scale, bias, out, n, d, h, wd, ci, lrelu_alpha);
-  return check_launch("conv3d_c4_fwd_kernel");
-}
 
 extern "C" int vp_conv3d_c4_wgrad(const float* x, const float* dy, float* gw, int n, int d, int h, int wd, int ci,
                                   vp_stream_t stream) {

@@ -72,7 +72,7 @@ def tensor_view(t, c=None, c_off=0):
         n, d, h, w, ct = t.shape
     c = ct - c_off if c is None else c
     v = VpTensor(t.data_ptr() + 4 * c_off, n, d, h, w, c, ct)
-    v._owner = t          # keeps the storage alive and lets the autotuner snapshot / restore an output it accumulates into
+    v._owner = t          # keeps the storage alive while the view is in use
     return v
 
 
@@ -86,10 +86,9 @@ _PROFILE = None         # list of (kind, algorithmic flops, start event, end eve
 _PROFILE_REPLAY = False
 
 
-def profile_engine(on, by_geometry=False, replay=False):
+def profile_engine(on, replay=False):
     """Starts / stops recording every tensor-core engine call (algorithmic FLOPs + GPU time).  Stopping returns
-    {'igemm' | 'wgrad': dict(calls, flops, ms)} for the whole-engine roofline of bench.py, or with by_geometry the same sums
-    per (kind, geometry key, engine).  Timing: CUDA events around the eager call on its launching stream, which for kernels
+    {'igemm' | 'wgrad': dict(calls, flops, ms)} for the whole-engine roofline of bench.py.  Timing: CUDA events around the eager call on its launching stream, which for kernels
     shorter than a launch costs on the host (ctypes + tensor-map encoding, ~25 us) measures the HOST, not the GPU; with
     replay=True every call is additionally captured four times into a CUDA graph and the replay is timed (GPU time only,
     operands L2-warm; calls that accumulate into their output are repeated too, so the step's numbers are garbage)."""
@@ -100,8 +99,8 @@ def profile_engine(on, by_geometry=False, replay=False):
     rec, _PROFILE = _PROFILE or [], None
     torch.cuda.synchronize()
     out = {}
-    for kind, flops, e0, e1, key, reps in rec:
-        d = out.setdefault((kind, key) if by_geometry else kind, dict(calls=0, flops=0.0, ms=0.0))
+    for kind, flops, e0, e1, reps in rec:
+        d = out.setdefault(kind, dict(calls=0, flops=0.0, ms=0.0))
         d['calls'] += 1
         d['flops'] += flops
         d['ms'] += e0.elapsed_time(e1) / reps
@@ -117,7 +116,7 @@ def _conv_flops(x_view, g, out_view):
     return 2.0 * out_view.n * out_view.d * out_view.h * out_view.w * out_view.c * x_view.c * taps
 
 
-def _profiled(kind, flops, call, key=None):
+def _profiled(kind, flops, call):
     if _PROFILE is None:
         return call()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -133,37 +132,30 @@ def _profiled(kind, flops, call, key=None):
         g.replay()
         e1.record()
         e1.synchronize()
-        _PROFILE.append((kind, flops, e0, e1, key, 4))
+        _PROFILE.append((kind, flops, e0, e1, 4))
         del g
         return
     e0.record()
     call()
     e1.record()
-    _PROFILE.append((kind, flops, e0, e1, key, 1))
-
-
-def _conv_key(x_view, g, n_pad, kc, out_view, act, extra):
-    return (x_view.n, x_view.d, x_view.h, x_view.w, x_view.c, out_view.n, out_view.d, out_view.h, out_view.w, out_view.c,
-            out_view.c == out_view.cstride, g.kd, g.kh, g.kw, g.sd, g.sh, g.sw, g.pd, g.ph, g.pw, g.transposed, n_pad, kc, act, extra)
+    _PROFILE.append((kind, flops, e0, e1, 1))
 
 
 def conv_igemm(x_view, g, wpacked, n_pad, kc, out_view, bias=None, act=ACT_NONE, alpha=0.0, split_k=1, accumulate=0):
     if 'igemm' in _SKIP:
         return
-    key = _conv_key(x_view, g, n_pad, kc, out_view, act, ('fwd', split_k))
     _profiled('igemm', _conv_flops(x_view, g, out_view),
               lambda: check(lib().vp_conv_igemm(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view), ptr(bias),
-                                                act, C.c_float(alpha), split_k, int(accumulate), stream_ptr())), key)
+                                                act, C.c_float(alpha), split_k, int(accumulate), stream_ptr())))
 
 
 def conv_igemm_actgrad(x_view, g, wpacked, n_pad, kc, out_view, act_output_addr, addend_addr, act, alpha=0.0, accumulate=0):
     if 'igemm' in _SKIP:
         return
-    key = _conv_key(x_view, g, n_pad, kc, out_view, act, ('actgrad', bool(addend_addr)))
     _profiled('igemm', _conv_flops(x_view, g, out_view),
               lambda: check(lib().vp_conv_igemm_actgrad(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view),
                                                         C.c_void_p(act_output_addr), C.c_void_p(addend_addr or 0), act,
-                                                        C.c_float(alpha), int(accumulate), stream_ptr())), key)
+                                                        C.c_float(alpha), int(accumulate), stream_ptr())))
 
 
 def tf32_residual(x):
@@ -176,7 +168,8 @@ def tf32_residual(x):
 
 def exact_mode():
     """VP_EXACT=1: every tensor-core convolution (forward, dgrad, wgrad) runs as three TF32 passes
-    hi*hi + lo*hi + hi*lo with fp32 accumulation = fp32-exact up to 2^-21 (debug / parity mode, ~3x the conv time)."""
+    hi*hi + lo*hi + hi*lo with fp32 accumulation = fp32-exact up to 2^-21 (debug / parity mode, ~3x the conv time).
+    A model reads it once, when it is built (`model.exact`)."""
     return os.environ.get('VP_EXACT', '0') == '1'
 
 
@@ -186,8 +179,7 @@ def conv_wgrad(x_view, dy_view, g, dwpacked, n_pad, kc, split_k=1):
     taps = g.kd * g.kh * g.kw / (float(g.sd * g.sh * g.sw) if g.transposed else 1.0)
     flops = 2.0 * dy_view.n * dy_view.d * dy_view.h * dy_view.w * dy_view.c * x_view.c * taps
     _profiled('wgrad', flops, lambda: check(lib().vp_conv_wgrad(C.byref(x_view), C.byref(dy_view), C.byref(g), ptr(dwpacked), n_pad, kc,
-                                                               split_k, stream_ptr())),
-              _conv_key(x_view, g, n_pad, kc, dy_view, 0, ('wgrad', split_k)))
+                                                               split_k, stream_ptr())))
 
 
 def eff_taps(k, kind):
@@ -212,14 +204,19 @@ def choose_n_pad(rows):
     return tiles * bn
 
 
+def pack_dims(k, ci_int, co, kind, layout):
+    """(n_pad, kc, floats) of the packed buffer of a [k][ci_int -> co] kernel in `layout`."""
+    rows, cols = (co, ci_int) if (layout & 3) == WLAYOUT_FWD else (ci_int, co)
+    n_pad, kc = choose_n_pad(rows), pad_to(cols, 32) // 32
+    return n_pad, kc, eff_taps(k, kind) * n_pad * kc * 32
+
+
 def pack_weights(w, k, ci_ref, co, kind, layout, ci_int=None, cmap=None, inv_scale=None, out=None):
     """Returns (wpacked, n_pad, kc)."""
     ci_int = ci_ref if ci_int is None else ci_int
-    rows, cols = (co, ci_int) if (layout & 3) == WLAYOUT_FWD else (ci_int, co)
-    n_pad, kc = choose_n_pad(rows), pad_to(cols, 32) // 32
-    taps = eff_taps(k, kind)
+    n_pad, kc, total = pack_dims(k, ci_int, co, kind, layout)
     if out is None:
-        out = torch.empty(taps * n_pad * kc * 32, device=w.device, dtype=torch.float32)
+        out = torch.empty(total, device=w.device, dtype=torch.float32)
     elif 'pack' in _SKIP:
         return out, n_pad, kc
     check(lib().vp_pack_weights(ptr(w), k[0], k[1], k[2], ci_ref, co, kind, layout, ptr(cmap), ci_int,
@@ -246,9 +243,7 @@ class PackPlan(object):
         self.keep = entries                                   # the table holds raw pointers: keep the tensors alive
         for j, (w, k, ci_ref, co, kind, layout, ci_int, cmap, inv_scale, out) in zip(jobs, entries):
             ci_int = ci_ref if ci_int is None else ci_int
-            rows, cols = (co, ci_int) if (layout & 3) == WLAYOUT_FWD else (ci_int, co)
-            n_pad, kc = choose_n_pad(rows), pad_to(cols, 32) // 32
-            total = eff_taps(k, kind) * n_pad * kc * 32
+            n_pad, kc, total = pack_dims(k, ci_int, co, kind, layout)
             assert out.numel() == total and w.is_contiguous()
             j.w, j.wpacked = w.data_ptr(), out.data_ptr()
             j.cmap = cmap.data_ptr() if cmap is not None else None
@@ -506,12 +501,6 @@ def scatter_clip(dclip, t_start, dvideo, clips, clip_len, pixels, video_batch, b
                                 batch_offset, stream_ptr()))
 
 
-def conv3d_c4_fwd(x, w, inv_scale, bias, out, n, d, h, wd, ci, alpha):
-    if 'c4fwd' in _SKIP:
-        return
-    check(lib().vp_conv3d_c4_fwd(ptr(x), ptr(w), ptr(inv_scale), ptr(bias), ptr(out), n, d, h, wd, ci, _f(alpha), stream_ptr()))
-
-
 def conv3d_c4_fwd_tc_ok(h, wd):
     """Shapes vp_conv3d_c4_fwd_tc tiles: L in {16, 8, 4} lines with h % L == 0 and three (L+2) x (wd+2) float4 planes <= 90 KB."""
     return wd + 2 <= 256 and any(h % L == 0 and 3 * (L + 2) * (wd + 2) * 16 <= 90 * 1024 for L in (16, 8, 4))
@@ -524,13 +513,17 @@ def conv3d_c4_fwd_tc(x, w, inv_scale, bias, out, n, d, h, wd, ci, alpha):
 
 
 def conv3d_c4_wgrad(x, dy, gw, n, d, h, wd, ci):
+    """The exact fp32 CUDA-core weight gradient of the first discriminator layer (any width)."""
     if 'c4wgrad' in _SKIP:
         return
-    # tensor cores unless the fp32-exact mode is on (the CUDA-core kernel is exact) or the width does not tile by 64
-    if wd % 64 == 0 and not exact_mode() and os.environ.get('VP_D0_WGRAD_CUDA_CORE', '0') != '1':
-        check(lib().vp_conv3d_c4_wgrad_tc(ptr(x), ptr(dy), ptr(gw), n, d, h, wd, ci, stream_ptr()))
-        return
     check(lib().vp_conv3d_c4_wgrad(ptr(x), ptr(dy), ptr(gw), n, d, h, wd, ci, stream_ptr()))
+
+
+def conv3d_c4_wgrad_tc(x, dy, gw, n, d, h, wd, ci):
+    """The same on the tensor cores (TF32 operands); needs wd % 64 == 0."""
+    if 'c4wgrad' in _SKIP:
+        return
+    check(lib().vp_conv3d_c4_wgrad_tc(ptr(x), ptr(dy), ptr(gw), n, d, h, wd, ci, stream_ptr()))
 
 
 def image_warp_fwd(im, im_cs, flow, out, out_cs, n, h, w, c):

@@ -65,81 +65,90 @@ class ConcatSpec(object):
 
 
 class ConvLayer(object):
-    """One convolution of the path: reference-layout parameters + packed tensor-core weights."""
+    """One convolution of the path (generator, posterior encoder and discriminator alike): reference-layout parameters +
+    packed tensor-core weights.  `spec` is the ConcatSpec of the input buffer, or (ci_ref, ci_int, cmap) given directly
+    (cmap None = identity).  `inv_scale` (optional device scalar, the spectral-norm sigma) divides the weights in every pack.
+    In the fp32-exact mode (`model.exact`) every call runs as three TF32 passes (conv3x) against the residual packs."""
 
-    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co):
+    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co, inv_scale=None):
         self.model, self.wname, self.bname = model, wname, bname
         self.k, self.kind, self.stride, self.pad, self.transposed = k, kind, stride, pad, transposed
-        self.spec, self.co = spec, co
-        self.ci_ref, self.ci_int = spec.ref_channels, spec.cstride
+        self.co, self.inv_scale = co, inv_scale
+        self.ci_ref, self.ci_int, cmap = (spec.ref_channels, spec.cstride, spec.cmap) if isinstance(spec, ConcatSpec) else spec
         if kind == L.WKIND_POOLED:
             self.ke = (1, k[1] + 1, k[2] + 1)
         elif kind == L.WKIND_UPSAMPLED:
             self.ke = (1, k[1] + 3, k[2] + 3)
         else:
             self.ke = k
+        # without a depth extent every leading dim of a buffer folds into n; a 3-D convolution keeps the depth axis
+        self.nd = 3 if (self.ke[0], stride[0], pad[0]) == (1, 1, 0) else 4
         self.geom = L.geom(self.ke, stride, pad, transposed)
-        self.cmap = torch.tensor(spec.cmap, dtype=torch.int32, device=model.device)
-        self.wp = None
-        self.n_pad = self.kc = None
+        self.cmap = None if cmap is None else torch.tensor(cmap, dtype=torch.int32, device=model.device)
+        self.wp, self.n_pad, self.kc = self._alloc(L.WLAYOUT_FWD)
+        self.wp_lo = self._alloc(L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL)[0] if model.exact else None
+        self.wpd = self.wpd_lo = None
 
-    def pack(self):
-        w = self.model.params[self.wname]
-        self.wp, self.n_pad, self.kc = L.pack_weights(w, self.k, self.ci_ref, self.co, self.kind, L.WLAYOUT_FWD,
-                                                      ci_int=self.ci_int, cmap=self.cmap, out=self.wp)
-        if L.exact_mode():      # fp32-exact 3xTF32 mode: the part of the weights the TF32 rounding dropped
-            self.wp_lo, _, _ = L.pack_weights(w, self.k, self.ci_ref, self.co, self.kind, L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL,
-                                              ci_int=self.ci_int, cmap=self.cmap, out=getattr(self, 'wp_lo', None))
+    def _alloc(self, layout):
+        n_pad, kc, total = L.pack_dims(self.k, self.ci_int, self.co, self.kind, layout)
+        return torch.empty(total, device=self.model.device), n_pad, kc
+
+    def _view(self, t):
+        return t.view((-1,) + tuple(t.shape[-self.nd:]))
 
     def prepare_backward(self):
         self.geom_bwd = L.geom(self.ke, self.stride, self.pad, not self.transposed)
-        self.wpd = self.dwp = None
-        self.pack_bwd()
-        self.dwp = torch.zeros(L.eff_taps(self.k, self.kind) * self.n_pad * self.kc * 32, device=self.model.device)
+        self.wpd, self.n_pad_d, self.kc_d = self._alloc(L.WLAYOUT_DGRAD)
+        self.wpd_lo = self._alloc(L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL)[0] if self.model.exact else None
+        self.dwp = torch.zeros_like(self.wp)
 
-    def pack_bwd(self):
+    def pack_jobs(self):
+        """PackPlan entries that fill every packed buffer of this layer from its reference-layout weights."""
         w = self.model.params[self.wname]
-        self.wpd, self.n_pad_d, self.kc_d = L.pack_weights(w, self.k, self.ci_ref, self.co, self.kind, L.WLAYOUT_DGRAD,
-                                                          ci_int=self.ci_int, cmap=self.cmap, out=getattr(self, 'wpd', None))
-        if L.exact_mode():
-            self.wpd_lo, _, _ = L.pack_weights(w, self.k, self.ci_ref, self.co, self.kind, L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL,
-                                               ci_int=self.ci_int, cmap=self.cmap, out=getattr(self, 'wpd_lo', None))
-
-    def dgrad(self, dy, dx, dy_c=None, accumulate=False):
-        """dx[.., ci_int] (+)= conv^T(dy): the same engine with the transposed flag flipped."""
-        dy4 = dy.view((-1,) + tuple(dy.shape[-3:]))
-        dyv = L.tensor_view(dy4, self.co if dy_c is None else dy_c)
-        dxv = L.tensor_view(dx.view((-1,) + tuple(dx.shape[-3:])), self.ci_int)
-        if L.exact_mode():
-            conv3x(dy4, dyv.c, self.geom_bwd, self.wpd, self.wpd_lo, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, 0.0,
-                   accumulate)
-            return
-        L.conv_igemm(dyv, self.geom_bwd, self.wpd, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, 0.0, 1 if accumulate else 0,
-                     accumulate)
-
-    def wgrad(self, x, dy, dy_c=None):
-        """grads[w] += dL/dw from ONE GEMM over every position of the (time-stacked) tensors."""
-        x4, dy4 = x.reshape((-1,) + tuple(x.shape[-3:])), dy.reshape((-1,) + tuple(dy.shape[-3:]))
-        xv = L.tensor_view(x4, self.ci_int)
-        dyv = L.tensor_view(dy4, self.co if dy_c is None else dy_c)
-        self.dwp.zero_()
-        L.conv_wgrad(xv, dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
-        if L.exact_mode():      # + x_lo^T dy + x^T dy_lo
-            L.conv_wgrad(L.tensor_view(L.tf32_residual(x4), self.ci_int), dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
-            L.conv_wgrad(xv, L.tensor_view(L.tf32_residual(dy4), dyv.c), self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
-        L.unpack_wgrad(self.dwp, self.k, self.ci_ref, self.co, self.kind, self.model.grads[self.wname], self.n_pad, self.kc,
-                       ci_int=self.ci_int, cmap=self.cmap)
+        bufs = ((L.WLAYOUT_FWD, self.wp), (L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL, self.wp_lo),
+                (L.WLAYOUT_DGRAD, self.wpd), (L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL, self.wpd_lo))
+        return [(w, self.k, self.ci_ref, self.co, self.kind, layout, self.ci_int, self.cmap, self.inv_scale, out)
+                for layout, out in bufs if out is not None]
 
     def fwd(self, x, out, out_off=0, out_c=None, act=L.ACT_NONE, alpha=0.0, split_k=0):
-        """x: stacked buffer [.., h, w, cstride] (4-D or 5-D torch tensor, leading dims folded into n)."""
-        x4 = x.view((-1,) + tuple(x.shape[-3:]))
-        xv = L.tensor_view(x4, self.ci_int)
-        ov = L.tensor_view(out.view((-1,) + tuple(out.shape[-3:])), self.co if out_c is None else out_c, out_off)
+        """x: stacked buffer [.., (d,) h, w, cstride] (any leading dims)."""
+        x = self._view(x)
+        xv = L.tensor_view(x, self.ci_int)
+        ov = L.tensor_view(self._view(out), self.co if out_c is None else out_c, out_off)
         bias = self.model.params[self.bname] if self.bname else None
-        if L.exact_mode():
-            conv3x(x4, self.ci_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, ov, bias, act, alpha)
+        if self.model.exact:
+            conv3x(x, self.ci_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, ov, bias, act, alpha)
             return
         L.conv_igemm(xv, self.geom, self.wp, self.n_pad, self.kc, ov, bias, act, alpha, split_k)
+
+    def dgrad(self, dy, dx, dy_c=None, accumulate=False, act_y=None, addend=None, act=L.ACT_NONE, alpha=0.0):
+        """dx[.., ci_int] (+)= conv^T(dy): the same engine with the transposed flag flipped.  With act_y, the output of the
+        activation `act` that produced this layer's input: dx = (conv^T(dy) + addend) * act'(act_y), fused into the epilogue."""
+        dy, dx = self._view(dy), self._view(dx)
+        dyv, dxv = L.tensor_view(dy, self.co if dy_c is None else dy_c), L.tensor_view(dx, self.ci_int)
+        aux = None if act_y is None else (act_y.data_ptr(), 0 if addend is None else addend.data_ptr(), act)
+        if self.model.exact:
+            conv3x(dy, dyv.c, self.geom_bwd, self.wpd, self.wpd_lo, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, alpha,
+                   accumulate, aux)
+        elif aux is None:
+            L.conv_igemm(dyv, self.geom_bwd, self.wpd, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, 0.0,
+                         1 if accumulate else 0, accumulate)
+        else:
+            L.conv_igemm_actgrad(dyv, self.geom_bwd, self.wpd, self.n_pad_d, self.kc_d, dxv, aux[0], aux[1], act, alpha,
+                                 2 if accumulate else 0)
+
+    def wgrad(self, x, dy, dy_c=None, dw=None):
+        """dw (default grads[w]) += dL/dw from ONE GEMM over every position of the (time-stacked) tensors."""
+        x, dy = self._view(x), self._view(dy)
+        xv = L.tensor_view(x, self.ci_int)
+        dyv = L.tensor_view(dy, self.co if dy_c is None else dy_c)
+        self.dwp.zero_()
+        L.conv_wgrad(xv, dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
+        if self.model.exact:      # + x_lo^T dy + x^T dy_lo
+            L.conv_wgrad(L.tensor_view(L.tf32_residual(x), self.ci_int), dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
+            L.conv_wgrad(xv, L.tensor_view(L.tf32_residual(dy), dyv.c), self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
+        L.unpack_wgrad(self.dwp, self.k, self.ci_ref, self.co, self.kind, self.model.grads[self.wname] if dw is None else dw,
+                       self.n_pad, self.kc, ci_int=self.ci_int, cmap=self.cmap)
 
 
 def conv3x(x, c, geom, wp, wp_lo, n_pad, kc, ov, bias, act, alpha, accumulate=False, aux=None):
@@ -350,6 +359,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise RuntimeError('video_prediction_b200 needs a CUDA device (sm_90a); there is no CPU fallback')
         L.lib()  # fail loudly if the CUDA library is missing
         self._check_supported()
+        self.exact = L.exact_mode()     # the arithmetic of every convolution of this model, fixed when its buffers are laid out
         hp = self.hparams
         # data parallelism (base_model.py:517-646): one process per GPU.  torchrun's env gives rank / world; with the
         # reference's `num_gpus` > 1 the batch in `inputs` is the GLOBAL batch and every rank takes its shard
@@ -715,7 +725,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['zc'] = self._z(S + 1, NB, nz)
             Bf['zh'] = self._z(S + 1, NB, nz)
             self._build_posterior()
-        self._pack_all()
+        self._plan_packs()
 
     def _build_posterior(self):
         hp = self.hparams
@@ -747,24 +757,15 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         Bf['eps'] = self._z(S, B, hp.nz)
         Bf['zprior'] = self._z(self.T - hp.context_frames, B, hp.nz)
 
+    def _plan_packs(self):
+        """One PackPlan over every packed buffer of the generator / encoder convolutions, built when the layers are and again
+        when prepare_backward has added the dgrad buffers; runs it once to fill the new buffers."""
+        self._pack_plan = L.PackPlan([job for c in self.convs for job in c.pack_jobs()])
+        self._pack_all()
+
     def _pack_all(self):
-        """Repacks every generator / encoder convolution weight after an optimizer step: one table-driven launch once all
-        packed buffers exist (the first call creates them layer by layer), per-layer calls in the fp32-exact mode."""
-        plan = getattr(self, '_pack_plan', None)
-        if plan is not None:
-            plan.run()
-            return
-        for c in self.convs:
-            c.pack()
-            if getattr(c, 'wpd', None) is not None:
-                c.pack_bwd()
-        if not L.exact_mode() and os.environ.get('VP_PACK_BATCH', '1') == '1' and all(getattr(c, 'wpd', None) is not None for c in self.convs):
-            entries = []
-            for c in self.convs:
-                w = self.params[c.wname]
-                entries.append((w, c.k, c.ci_ref, c.co, c.kind, L.WLAYOUT_FWD, c.ci_int, c.cmap, None, c.wp))
-                entries.append((w, c.k, c.ci_ref, c.co, c.kind, L.WLAYOUT_DGRAD, c.ci_int, c.cmap, None, c.wpd))
-            self._pack_plan = L.PackPlan(entries)
+        """Repacks every generator / encoder convolution weight (after an optimizer step or set_params): one launch."""
+        self._pack_plan.run()
 
     # ------------------------------------------------------------------ inputs
     def set_inputs(self, inputs, noise=None, sampling=None):

@@ -42,19 +42,17 @@ def _ceil4(v):
 
 
 class SNLayer(object):
-    """A spectrally-normalised conv3d (or the final dense) of the video discriminator."""
+    """A spectrally-normalised conv3d / conv2d (or the final dense) of a discriminator tower: spectral norm forward and
+    backward around a ConvLayer whose packs divide the weights by sigma.  `spec` = (ci_ref, ci_int, cmap) of the input."""
 
-    def __init__(self, model, scope, name, k, stride, cin_ref, cin_int, cmap, co, is_fc=False, fc_in=0, two_d=False):
-        self.m, self.is_fc = model, is_fc
-        self.k, self.stride, self.co = k, stride, co
-        self.two_d = two_d                          # image discriminator: conv2d kernels [k,k,ci,co], no temporal extent
-        self.k3 = (1, k, k) if two_d else (k, k, k)
-        self.cin_ref, self.cin_int = cin_ref, cin_int
-        sub = 'dense' if is_fc else ('conv2d' if two_d else 'conv3d')
+    def __init__(self, model, scope, name, k, stride, spec, co, is_fc=False, fc_in=0, two_d=False):
+        self.m, self.is_fc, self.co = model, is_fc, co
+        sub = 'dense' if is_fc else ('conv2d' if two_d else 'conv3d')   # image discriminator: conv2d kernels [k,k,ci,co]
         self.wname = '%s/%s/%s/kernel' % (scope, name, sub)
         self.uname = '%s/%s/%s/u' % (scope, name, sub)
         self.bname = '%s/%s/%s/bias' % (scope, name, sub)
-        self.rows = fc_in if is_fc else int(np.prod(self.k3)) * cin_ref
+        self.k3, self.stride = ((1, k, k) if two_d else (k, k, k)), stride
+        self.rows = fc_in if is_fc else int(np.prod(self.k3)) * spec[0]
         self.cols = co
         dev = model.device
         z = lambda *s: torch.zeros(*s, device=dev, dtype=torch.float32)
@@ -62,12 +60,17 @@ class SNLayer(object):
         self.gs, self.gt = z(self.cols), z(self.rows)
         self.gwbar = z(self.rows * self.cols)
         self.u_next = z(self.cols)
-        self.cmap = None if cmap is None else torch.tensor(cmap, dtype=torch.int32, device=dev)
-        if not is_fc:
-            pad = (0, 1, 1) if two_d else (1, 1, 1)        # tf.pad of 1 on H,W (and T for conv3d) + VALID (networks.py:38-43, 76-81)
-            self.geom = L.geom(self.k3, stride, pad, False)
-            self.geom_t = L.geom(self.k3, stride, pad, True)
-            self.wp = self.wpd = self.dwp = None
+        if is_fc:
+            return
+        from .savp_model import ConvLayer      # savp_model imports this module for TrainMixin
+        pad = (0, 1, 1) if two_d else (1, 1, 1)        # tf.pad of 1 on H,W (and T for conv3d) + VALID (networks.py:38-43, 76-81)
+        self.conv = ConvLayer(model, self.wname, self.bname, self.k3, L.WKIND_PLAIN, stride, pad, False, spec, co,
+                              inv_scale=self.sigma)
+        self.conv.prepare_backward()
+        self.cin_ref, self.cin_int, self.cmap, self.geom = self.conv.ci_ref, self.conv.ci_int, self.conv.cmap, self.conv.geom
+        # the first video layer (3 colour channels as float4 voxels -> 32, 3x3x3) has its own kernels (csrc/d0_layer.cu): with 4
+        # channels per tap the generic engine would pad every operand to 32 channels and issue one K = 8 MMA per pipeline stage
+        self.first_layer_3to32 = not two_d and k == 3 and tuple(stride) == (1, 1, 1) and self.cin_ref <= 3 and co == 32
 
     @property
     def sigma(self):
@@ -77,87 +80,31 @@ class SNLayer(object):
         P = self.m.params
         L.spectral_norm_fwd(P[self.wname], P[self.uname], self.rows, self.cols, self.v, self.s, self.u_new, self.scal)
 
-    def pack(self):
-        if self.is_fc:
-            return
-        w = self.m.params[self.wname]
-        kk = self.k3
-        self.wp, self.n_pad, self.kc = L.pack_weights(w, kk, self.cin_ref, self.co, L.WKIND_PLAIN, L.WLAYOUT_FWD,
-                                                      ci_int=self.cin_int, cmap=self.cmap, inv_scale=self.sigma, out=self.wp)
-        self.wpd, self.n_pad_d, self.kc_d = L.pack_weights(w, kk, self.cin_ref, self.co, L.WKIND_PLAIN, L.WLAYOUT_DGRAD,
-                                                          ci_int=self.cin_int, cmap=self.cmap, inv_scale=self.sigma, out=self.wpd)
-        if L.exact_mode():
-            self.wp_lo, _, _ = L.pack_weights(w, kk, self.cin_ref, self.co, L.WKIND_PLAIN, L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL,
-                                              ci_int=self.cin_int, cmap=self.cmap, inv_scale=self.sigma, out=getattr(self, 'wp_lo', None))
-            self.wpd_lo, _, _ = L.pack_weights(w, kk, self.cin_ref, self.co, L.WKIND_PLAIN, L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL,
-                                               ci_int=self.cin_int, cmap=self.cmap, inv_scale=self.sigma, out=getattr(self, 'wpd_lo', None))
-        if self.dwp is None:
-            self.dwp = torch.zeros(int(np.prod(self.k3)) * self.n_pad * self.kc * 32, device=w.device)
-
-    @property
-    def cuda_core(self):
-        """First layer (3 colour channels -> 32): runs on the CUDA-core kernels of csrc/discrim.cu.  With 4 channels per
-        tap the generic tensor-core engine would pad every operand to 32 channels and issue one K = 8 MMA per pipeline stage
-        (VP_D0_CUDA_CORE=0 selects the engine for comparison)."""
-        if os.environ.get('VP_D0_CUDA_CORE', '1') != '1':
-            return False
-        return (not self.is_fc) and not self.two_d and self.k == 3 and tuple(self.stride) == (1, 1, 1) and self.cin_ref <= 3 and self.co == 32
-
     def fwd(self, x, out):
-        # the first layer has its own tensor-core kernels (csrc/d0_layer.cu): float4 voxel rows are tensor-core operands as they lie
-        # -- forward: overlapping rows x[v-1 .. v+2] = the K = 16 operand of a kernel row, 18 MMAs per 128 voxels against
-        # 108 on the generic engine; weight gradient: the overlapping voxels of a halo row as the (dx, ci) x voxel operand.
-        # The fp32-exact mode runs the generic engine (3xTF32) and the exact CUDA-core weight gradient.
-        if self.cuda_core and not L.exact_mode():
+        # first layer: overlapping float4 voxel rows x[v-1 .. v+2] are the K = 16 operand of a kernel row, 18 MMAs per 128
+        # voxels against 108 on the generic engine; the fp32-exact mode and shapes the kernel does not tile take the engine
+        n, d, h, w = x.shape[:4]
+        if self.first_layer_3to32 and not self.m.exact and L.conv3d_c4_fwd_tc_ok(h, w):
             P = self.m.params
-            n, d, h, w = x.shape[:4]
-            if os.environ.get('VP_D0_FWD_CUDA_CORE', '0') == '1':
-                L.conv3d_c4_fwd(x, P[self.wname], self.sigma, P[self.bname], out, n, d, h, w, self.cin_ref, 0.1)
-                return
-            if os.environ.get('VP_D0_FWD_ENGINE', '0') != '1' and L.conv3d_c4_fwd_tc_ok(h, w):
-                L.conv3d_c4_fwd_tc(x, P[self.wname], self.sigma, P[self.bname], out, n, d, h, w, self.cin_ref, 0.1)
-                return
-        if L.exact_mode():
-            from .savp_model import conv3x
-            conv3x(x, self.cin_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, L.tensor_view(out, self.co),
-                   self.m.params[self.bname], L.ACT_LRELU, 0.1)
+            L.conv3d_c4_fwd_tc(x, P[self.wname], self.sigma, P[self.bname], out, n, d, h, w, self.cin_ref, 0.1)
             return
-        L.conv_igemm(L.tensor_view(x, self.cin_int), self.geom, self.wp, self.n_pad, self.kc, L.tensor_view(out, self.co),
-                     self.m.params[self.bname], L.ACT_LRELU, 0.1)
+        self.conv.fwd(x, out, act=L.ACT_LRELU, alpha=0.1)
 
     def dgrad(self, dy, dx, act_y=None, addend=None):
         """dx = conv^T(dy); with act_y: dx = (conv^T(dy) + addend) * lrelu'(act_y) -- the backward of the previous
         layer's leaky relu fused into the epilogue."""
-        dyv, dxv = L.tensor_view(dy, self.co), L.tensor_view(dx, self.cin_int)
-        if L.exact_mode():
-            from .savp_model import conv3x
-            aux = None if act_y is None else (act_y.data_ptr(), addend.data_ptr() if addend is not None else 0, L.ACT_LRELU)
-            conv3x(dy, self.co, self.geom_t, self.wpd, self.wpd_lo, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, 0.1, aux=aux)
-            return
-        if act_y is None:
-            L.conv_igemm(dyv, self.geom_t, self.wpd, self.n_pad_d, self.kc_d, dxv, None, L.ACT_NONE, 0.0, 0)
-        else:
-            L.conv_igemm_actgrad(dyv, self.geom_t, self.wpd, self.n_pad_d, self.kc_d, dxv, act_y.data_ptr(),
-                                 addend.data_ptr() if addend is not None else 0, L.ACT_LRELU, 0.1)
+        self.conv.dgrad(dy, dx, act_y=act_y, addend=addend, act=L.ACT_LRELU, alpha=0.1)
 
     def wgrad(self, x, dy):
-        """dW += SN-backward(dL/dWbar) with dL/dWbar from the tensor-core wgrad GEMM."""
-        m = self.m
-        if self.cuda_core:
-            n, d, h, w = x.shape[:4]
-            self.gwbar.zero_()
-            L.conv3d_c4_wgrad(x, dy, self.gwbar, n, d, h, w, self.cin_ref)
-            self.sn_backward()
-            return
-        self.dwp.zero_()
-        xv, dyv = L.tensor_view(x, self.cin_int), L.tensor_view(dy, self.co)
-        L.conv_wgrad(xv, dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
-        if L.exact_mode():
-            L.conv_wgrad(L.tensor_view(L.tf32_residual(x.contiguous()), self.cin_int), dyv, self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
-            L.conv_wgrad(xv, L.tensor_view(L.tf32_residual(dy.contiguous()), self.co), self.geom, self.dwp, self.n_pad, self.kc, split_k=0)
+        """dW += SN-backward(dL/dWbar).  First layer: the overlapping voxels of a halo row are the tensor-core operand
+        (w % 64 == 0); the fp32-exact mode and other widths take the exact CUDA-core kernel."""
         self.gwbar.zero_()
-        L.unpack_wgrad(self.dwp, self.k3, self.cin_ref, self.co, L.WKIND_PLAIN, self.gwbar, self.n_pad, self.kc,
-                       ci_int=self.cin_int, cmap=self.cmap)
+        if self.first_layer_3to32:
+            n, d, h, w = x.shape[:4]
+            wgrad = L.conv3d_c4_wgrad_tc if (not self.m.exact and w % 64 == 0) else L.conv3d_c4_wgrad
+            wgrad(x, dy, self.gwbar, n, d, h, w, self.cin_ref)
+        else:
+            self.conv.wgrad(x, dy, dw=self.gwbar)
         self.sn_backward()
 
     def sn_backward(self):
@@ -235,19 +182,21 @@ class TrainMixin(object):
             layers = VIDEO_D_LAYERS if kind == 'video' else IMAGE_D_LAYERS
             clip_len = hp.clip_length if kind == 'video' else 1
             net = dict(tw, layers=[], feat=[], dfeat=[], dcd=[], clip_len=clip_len)
-            cin_ref, cin_int, cmap = C, 4, list(range(C)) + [-1] * (4 - C)
+            spec = (C, 4, list(range(C)) + [-1] * (4 - C))      # colour channels stored as float4 voxels
             nb = 2 * B
             net['clip'] = z(nb, clip_len, H, W, 4)
             net['dclip'] = z(nb, clip_len, H, W, 4)
             for (name, mult, k, st), shp in zip(layers, shapes):
                 co = hp.ndf * mult
-                net['layers'].append(SNLayer(self, scope, name, k, st, cin_ref, cin_int, cmap, co, two_d=(kind == 'image')))
+                net['layers'].append(SNLayer(self, scope, name, k, st, spec, co, two_d=(kind == 'image')))
                 net['feat'].append(z(nb, *shp))
                 net['dfeat'].append(z(nb, *shp))
                 net['dcd'].append(z(B, *shp))
-                cin_ref, cin_int, cmap = co, co, None
+                spec = (co, co, None)
             f = int(np.prod(shapes[-1]))
-            net['fc'] = SNLayer(self, scope, 'sn_fc4', 1, None, f, f, None, 1, is_fc=True, fc_in=f)
+            net['fc'] = SNLayer(self, scope, 'sn_fc4', 1, None, None, 1, is_fc=True, fc_in=f)
+            # every weight pack of the tower in one launch, run after the tower's spectral-norm forwards wrote sigma
+            net['pack'] = L.PackPlan([job for lay in net['layers'] for job in lay.conv.pack_jobs()])
             net['logits'] = z(nb)
             net['dlogits'] = z(nb)
             net['tstart'] = torch.zeros(2, B, dtype=torch.int32, device=self.device)
@@ -307,13 +256,13 @@ class TrainMixin(object):
         self._scal_host = torch.zeros(4, dtype=torch.float32).pin_memory()
         for c in self.convs:
             c.prepare_backward()
+        self._plan_packs()
 
     # ------------------------------------------------------------------ discriminator forward / backward
-    def _d_sn_and_pack(self):
-        for net in self.dnets.values():
-            for lay in net['layers'] + [net['fc']]:
-                lay.sn_forward()
-                lay.pack()
+    def _d_sn_and_pack(self, net):
+        for lay in net['layers'] + [net['fc']]:
+            lay.sn_forward()
+        net['pack'].run()
 
     def _d_gather(self, net, which, t_real, t_fake, fake_off, rows_real=True):
         """Fills net['clip']: rows [0,B) real clip (optional), rows [B,2B) fake clip."""
@@ -619,7 +568,7 @@ class TrainMixin(object):
             self.redraw_step_randomness(noise, sampling)      # resident inputs: fresh eps / z_prior / sampling mask per step
         if not staged:
             self.stage_step(self._shard_noise(noise))
-        if self.use_cuda_graph and not staged and self._eager_steps >= 1 and not L.exact_mode():
+        if self.use_cuda_graph and not staged and self._eager_steps >= 1 and not self.exact:
             # the device part of the step (~1.5 k launches, no host sync) is captured once and replayed
             if self._graph is None:
                 try:
@@ -679,9 +628,8 @@ class TrainMixin(object):
         def d_prepare(net):
             # spectral norm + weight packing of one tower (dozens of tiny dependent launches): independent of the generator
             # forward, so it runs as a parallel graph branch underneath it
+            self._d_sn_and_pack(net)
             for lay in net['layers'] + [net['fc']]:
-                lay.sn_forward()
-                lay.pack()
                 lay.u_next.copy_(lay.u_new)     # UPDATE_OPS (ops.py:1046-1048): u' of the start-of-step weights
 
         self._run_concurrent([lambda: self.generator_forward(collect=False)] +
@@ -709,7 +657,8 @@ class TrainMixin(object):
             L.adam(self.d_flat, self.d_grad, self.d_m, self.d_v, self.d_flat.numel(), self.step_scalars[0:1], hp.beta1, hp.beta2,
                    1.0 / world)
             # post-update discriminator forward (fresh reads of the updated variables, tf_utils.replace_read_ops)
-            self._d_sn_and_pack()
+            for net in self.dnets.values():
+                self._d_sn_and_pack(net)
         # ---- generator loss seeds
         G['dgen'].zero_()
         self.g_grad.zero_()

@@ -228,6 +228,24 @@ int vp_flow_apply_bwd(const float* image, const float* flows, int flows_cstride,
                       const float* d_b, int d_b_cstride, float* dimage, float* dflows, int n, int h, int w, int nk,
                       vp_stream_t stream);
 
+/* Pixel distributions (savp_model.py:408-410, 598-621, 648-653), one whole time step, forward only (no gradient in any
+ * mode).  Per row n and channel c < d of the [n][h][w][*] channels-last maps:
+ *   p        = (gen_prev == NULL || sel[n]) ? pix_gt : gen_prev                    (:409; gen_prev = NULL at t = 0)
+ *   slot_k   = CDNA_k(p) (kernels [n][kh*kw][nk], SYMMETRIC padding, as vp_cdna_apply) or, when kernels is NULL,
+ *              image_warp(p, flows_k) (flows channel k = x, nk + k = y, as vp_flow_apply),            k < nk (:598-604)
+ *   slot_nk  = p,  slot_nk+1 = pix_first,  slot_nk+2 = p (the scratch slot takes the map, :606-621)
+ *   g        = sum_l masks[l] * slot_l (masks: the softmax masks vp_composite wrote, l < nk + 3)      (:648-652)
+ *   gen      = g / sum_{h,w} g, without an epsilon                                                  (:653)
+ * pix_gt / pix_first share pix_cstride, gen_prev / gen share gen_cstride; slot l of channel c is written at
+ * transformed[(n*h*w + p) * transformed_cstride + l * slot_stride + c].  All strides are multiples of 4; only channels
+ * c < d are written.  Exactly one of kernels and flows is given; nk + 3 <= 8.  The plane sum is order-fixed (one
+ * 8-CTA cluster per (n, c) plane, partials added through DSMEM in rank order): identical inputs give identical bits. */
+int vp_pix_distrib_fwd(const int32_t* sel, const float* pix_gt, const float* pix_first, int pix_cstride,
+                       const float* gen_prev, const float* kernels, const float* flows, int flows_cstride,
+                       const float* masks, int masks_cstride, float* gen, int gen_cstride, float* transformed,
+                       int transformed_cstride, int slot_stride, int n, int h, int w, int d, int kh, int kw, int nk,
+                       vp_stream_t stream);
+
 /* ---- losses (losses.py:6-67): out[0] += value; optional gradient = grad_scale * d value / d pred -------- */
 int vp_pixel_loss(const float* pred, int pred_cstride, const float* target, int target_cstride, float* dpred,
                   int dpred_cstride, long long rows, int c, int mode /*bit 0: 0 = L1, 1 = L2; bit 1: dpred += instead of =*/, long long mean_count,

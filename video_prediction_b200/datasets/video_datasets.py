@@ -3,7 +3,8 @@
 raw uint8 frames) and the KTH format (`KTHVideoDataset`, kth_dataset.py:16-50: one Example per clip, a variable-length list
 of raw frames).  Constructor, hparams, file discovery, filtering, sub-sequence sampling (time shift, frame skip, macro
 actions) and batching follow base_dataset.py:12-312; `make_batch(batch_size)` returns one batch per call as a dict of
-numpy arrays (`images` [B,T,H,W,C] float32 in [0,1], `actions` [B,T-1,A], `states` [B,T,S]) -- what the model's
+numpy arrays (`images` [B,T,H,W,C] float32 in [0,1], `actions` [B,T-1,A], `states` [B,T,S], and for BAIR records with
+designated pixels `object_pos` [B,T,2D] and `pix_distribs` [B,T,H,W,D]) -- what the model's
 `build_graph` / `train_step` take -- and raises StopIteration after `num_epochs` passes."""
 from __future__ import annotations
 
@@ -172,6 +173,24 @@ class BaseVideoDataset(object):
         return {k: np.stack([np.asarray(r[k], dtype=np.float32) for r in rows]) for k in rows[0]}
 
 
+def pixel_distribution(pos, height, width):
+    """tf_utils.pixel_distribution (tf_utils.py:562-585) in float32: pos [N,2] = (y, x) -> [N,H,W] maps with bilinear
+    weights on the four neighbours of the position.  Like the reference, each neighbour is a one-hot of the FLAT index
+    y*W + x over H*W entries: x = W lands on column 0 of the next row, and an index outside [0, H*W) adds nothing."""
+    pos = np.asarray(pos, np.float32)
+    n = pos.shape[0]
+    y, x = pos[:, 0], pos[:, 1]
+    x0, y0 = np.floor(x).astype(np.int64), np.floor(y).astype(np.int64)
+    x1, y1 = x0 + 1, y0 + 1
+    x0f, x1f, y0f, y1f = (v.astype(np.float32) for v in (x0, x1, y0, y1))
+    out = np.zeros((n, height * width), np.float32)
+    for idx, wgt in ((y0 * width + x0, (x1f - x) * (y1f - y)), (y1 * width + x0, (x1f - x) * (y - y0f)),
+                     (y0 * width + x1, (x - x0f) * (y1f - y)), (y1 * width + x1, (x - x0f) * (y - y0f))):
+        ok = (idx >= 0) & (idx < height * width)
+        np.add.at(out, (np.nonzero(ok)[0], idx[ok]), wgt[ok])
+    return out.reshape(n, height, width)
+
+
 def _crop_or_pad(video, th, tw):
     """tf.image.resize_image_with_crop_or_pad on [T,H,W,C]: centred crop and / or zero pad."""
     _, h, w, _ = video.shape
@@ -281,7 +300,8 @@ class VarLenFeatureVideoDataset(BaseVideoDataset):
 
 class SoftmotionVideoDataset(VideoDataset):
     """BAIR robot pushing (softmotion_dataset.py:10-82): frames under '%d/image_aux1/encoded' (or image_view0), optional
-    '%d/endeffector_pos' (3) and '%d/action' (4) with use_state."""
+    '%d/endeffector_pos' (3) and '%d/action' (4) with use_state, and '%d/object_pos' (2D floats: the (y, x) positions of D
+    designated pixels) when the records have it, which also yields their maps as `pix_distribs` [T,H,W,D]."""
 
     def __init__(self, *args, **kwargs):
         super(SoftmotionVideoDataset, self).__init__(*args, **kwargs)
@@ -299,7 +319,27 @@ class SoftmotionVideoDataset(VideoDataset):
         if self.hparams.use_state:
             self.state_like_names_and_shapes['states'] = ('%d/endeffector_pos', (3,))
             self.action_like_names_and_shapes['actions'] = ('%d/action', (4,))
+        if any(re.match(r'\d+/object_pos$', name) for name in self._first):       # softmotion_dataset.py:41-42
+            self.state_like_names_and_shapes['object_pos'] = ('%d/object_pos', None)
         self._check_or_infer_shapes()
+        if 'object_pos' in self.state_like_names_and_shapes:
+            h, w, _ = self.state_like_names_and_shapes['images'][1]
+            npos = self.state_like_names_and_shapes['object_pos'][1][0]
+            if npos % 2:
+                raise ValueError('object_pos holds (y, x) pairs; got %d values per frame' % npos)
+            crop, scale = self.hparams.crop_size, self.hparams.scale_size
+            side = scale or crop or min(h, w)
+            if (crop or scale) and (side, side) != (h, w):
+                raise NotImplementedError('object_pos with crop_size / scale_size changing the %dx%d frames: how the positions '
+                                          'map is not defined' % (h, w))
+
+    def parse(self, example):
+        state_like, action_like = super(SoftmotionVideoDataset, self).parse(example)
+        if 'object_pos' in state_like:                                      # softmotion_dataset.py:59-68
+            h, w, _ = self.state_like_names_and_shapes['images'][1]
+            pos = state_like['object_pos'].reshape(len(state_like['object_pos']), -1, 2)
+            state_like['pix_distribs'] = np.stack([pixel_distribution(pos[:, i], h, w) for i in range(pos.shape[1])], axis=-1)
+        return state_like, action_like
 
     def get_default_hparams_dict(self):
         d = super(SoftmotionVideoDataset, self).get_default_hparams_dict()

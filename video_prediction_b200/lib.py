@@ -358,6 +358,15 @@ def composite(logits, logits_cs, layers_addr, layers_cs, masks, masks_cs, gen, p
                              C.c_longlong(positions), num_layers, stream_ptr()))
 
 
+def pix_distrib_fwd(sel, pix_gt_addr, pix_first_addr, pix_cs, gen_prev_addr, kernels, flows, flows_cs, masks, masks_cs,
+                    gen_addr, gen_cs, tr_addr, tr_cs, slot_stride, n, h, w, d, kh, kw, nk):
+    """One time step of the pixel-distribution path (vp_pix_distrib_fwd); addresses are ints (0 = NULL) so that callers can
+    pass channel slices of concat buffers.  Exactly one of `kernels` (CDNA) and `flows` is a tensor."""
+    check(lib().vp_pix_distrib_fwd(ptr(sel), C.c_void_p(pix_gt_addr), C.c_void_p(pix_first_addr), pix_cs, C.c_void_p(gen_prev_addr),
+                                   ptr(kernels), ptr(flows), flows_cs, ptr(masks), masks_cs, C.c_void_p(gen_addr), gen_cs,
+                                   C.c_void_p(tr_addr), tr_cs, slot_stride, n, h, w, d, kh, kw, nk, stream_ptr()))
+
+
 # ---------------------------------------------------------------------------------- backward / losses / optimizer
 def _srcs(srcs):
     """srcs: list of (address:int, cstride:int) gradient sources to be summed."""

@@ -352,8 +352,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
     # ------------------------------------------------------------------ build
     def build_graph(self, inputs):
         """inputs: dict with 'images' [B,T,H,W,C] (torch / numpy, batch-major as in base_model.py:467)
-        and optionally 'actions' [B,T-1,A].  Allocates parameters (reference initialisers) unless
-        `set_params` was called, and all activation buffers."""
+        and optionally 'actions' [B,T-1,A] and 'pix_distribs' [B,T,H,W,D] (D designated-pixel probability maps, moved
+        with the images: gen_pix_distribs / transformed_pix_distribs in `outputs`).  Allocates parameters (reference
+        initialisers) unless `set_params` was called, and all activation buffers."""
         super(SAVPVideoPredictionModel, self).build_graph(inputs)
         if not torch.cuda.is_available():
             raise RuntimeError('video_prediction_b200 needs a CUDA device (sm_90a); there is no CPU fallback')
@@ -380,6 +381,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise ValueError('images have %d frames, sequence_length is %d' % (T, hp.sequence_length))
         self.B, self.T, self.H, self.W, self.C = B, hp.sequence_length, H, W, C
         self.A = int(inputs['actions'].shape[-1]) if 'actions' in inputs else 0
+        self.D = self._pix_distribs_depth(inputs)
         self.S = self.T - 1
         self.Zc = self.A + (hp.nz if hp.nz else 0)
         self.NB = 2 * B if hp.nz else B
@@ -410,6 +412,19 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             self._build_training()
         self.built = True
         self.set_inputs(inputs)
+
+    @staticmethod
+    def _pix_distribs_depth(inputs):
+        """D of inputs['pix_distribs'] [B,T,H,W,D] (0 without the key); the maps must cover the images' frames."""
+        if 'pix_distribs' not in inputs:
+            return 0
+        pd, im = inputs['pix_distribs'], inputs['images']
+        if len(pd.shape) != 5 or tuple(pd.shape[:4]) != tuple(im.shape[:4]):
+            raise ValueError('pix_distribs must be [B, T, H, W, D] with B, T, H, W of the images %s, got %s'
+                             % (tuple(im.shape), tuple(pd.shape)))
+        if int(pd.shape[4]) < 1:
+            raise ValueError('pix_distribs need at least one designated pixel (D >= 1), got shape %s' % (tuple(pd.shape),))
+        return int(pd.shape[4])
 
     def _alloc_params(self):
         """Flat fp32 buffers (one per optimizer: generator / discriminator, base_model.py:486-487) with
@@ -715,6 +730,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         Bf['img'] = self._z(S, NB, H, W, 4)
         Bf['x'] = self._z(self.T, NB, H, W, 4)
         Bf['sel'] = torch.ones(S, NB, device=self.device, dtype=torch.int32)
+        if self.D:
+            # pixel distributions (savp_model.py:408-410, 598-653): ground truth, generated maps and the nlayers transformed
+            # maps of every channel, each map padded to Dp channels
+            Dp = _ceil4(self.D)
+            Bf['pix'] = self._z(self.T, NB, H, W, Dp)
+            Bf['gpix'] = self._z(S, NB, H, W, Dp)
+            Bf['tpix'] = self._z(S, NB, H, W, self.nlayers * Dp)
         if Zc:
             Bf['zvec'] = self._z(S, NB, _ceil4(Zc))
         if hp.nz:
@@ -792,6 +814,14 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['zvec'][:, :B, :self.A] = act
             if self.NB > B:
                 Bf['zvec'][:, B:, :self.A] = act
+        if self._pix_distribs_depth(inputs) != self.D:
+            raise ValueError('the model was built %s pix_distribs; the inputs must match'
+                             % ('with %d-channel' % self.D if self.D else 'without'))
+        if self.D:
+            pd = torch.as_tensor(inputs['pix_distribs']).to(dev, torch.float32)[:, :T].permute(1, 0, 2, 3, 4)
+            Bf['pix'][:, :B, ..., :self.D] = pd
+            if self.NB > B:
+                Bf['pix'][:, B:, ..., :self.D] = pd
         sel = torch.ones(S, self.NB, dtype=torch.int32)
         n_free = S - hp.context_frames
         if sampling is None:
@@ -1080,6 +1110,14 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         self.conv_masks.fwd(mk, Bf['mlog'][t], out_c=self.nlayers)
         L.composite(Bf['mlog'][t], 8, mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, Bf['masks'][t], 8, Bf['gen'][t],
                     NB * HW, self.nlayers)
+        if self.D:
+            # pixel distributions (savp_model.py:408-410, 598-621, 648-653): same selection, transformation and masks
+            Dp = Bf['gpix'].shape[-1]
+            L.pix_distrib_fwd(Bf['sel'][t], Bf['pix'][t].data_ptr(), Bf['pix'][0].data_ptr(), Dp,
+                              Bf['gpix'][t - 1].data_ptr() if t else 0, None if self.flow else Bf['kern'][t],
+                              Bf['flows'][t] if self.flow else None, Bf['flows'].shape[-1] if self.flow else 0,
+                              Bf['masks'][t], 8, Bf['gpix'][t].data_ptr(), Dp, Bf['tpix'][t].data_ptr(), self.nlayers * Dp, Dp,
+                              NB, H, W, self.D, kh, kw, nk)
 
     def generator_forward(self, collect=True):
         hp = self.hparams
@@ -1189,5 +1227,15 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             out['gen_images'] = gen.permute(1, 0, 2, 3, 4)
             out['transformed_images'] = tr.permute(1, 0, 2, 3, 4, 5)
             out['masks'] = masks.permute(1, 0, 2, 3, 4, 5)
+        if self.D:
+            D, S, NB, H, W = self.D, self.S, self.NB, self.H, self.W
+            gpix = Bf['gpix'][..., :D]                                                             # [S,NB,H,W,D]
+            tpix = Bf['tpix'].view(S, NB, H, W, nlay, -1)[..., :D].transpose(-1, -2)               # [S,NB,H,W,D,L]
+            if self.hparams.nz:
+                out['gen_pix_distribs_enc'] = gpix[:, :B].permute(1, 0, 2, 3, 4)
+                out['transformed_pix_distribs_enc'] = tpix[:, :B].permute(1, 0, 2, 3, 4, 5)
+                gpix, tpix = gpix[:, B:], tpix[:, B:]
+            out['gen_pix_distribs'] = gpix.permute(1, 0, 2, 3, 4)
+            out['transformed_pix_distribs'] = tpix.permute(1, 0, 2, 3, 4, 5)
         self.outputs = out
         self.gen_images = out['gen_images']

@@ -5,7 +5,7 @@
 //
 // Operands are fp32 in HBM/shared memory and are consumed as TF32 by the tensor cores with fp32 accumulation in
 // registers.  Activation tiles are fetched with 5-D TMA boxes straight from the NDHWC tensor: a box of bw x bh x bd x bn
-// output positions is one 128-row (64-row for wgrad) operand tile whose rows are 32 channels = 128 bytes, written by TMA
+// positions is one 128-row (64-row for the wgrad's dy) operand tile whose rows are 32 channels = 128 bytes, written by TMA
 // with the 128-byte swizzle.  A filter tap is a coordinate shift of the box; TMA zero-fills out-of-bounds rows/channels,
 // which *is* the convolution's zero padding.  Strided convolutions read one of s_d*s_h*s_w "parity" sub-lattices of the
 // input (one tensor map each); transposed convolutions (upsample_conv2d forward, dgrad of strided convs) are split into
@@ -14,8 +14,10 @@
 // Forward / dgrad: both operands are K-major (channels contiguous), which is what wgmma needs for TF32: warpgroup 0 is
 // the TMA producer, warpgroups 1 and 2 each issue wgmma.m64nBNk8 on one 64-row half of the 128-pixel tile and run the
 // epilogue (bias / activation / fused activation gradient) from their accumulator registers.
-// Weight gradient: GEMM-K is the pixel dimension, so both shared-memory tiles are MN-major, which wgmma does not accept
-// for TF32; eight warps read their fragments from the swizzled TMA tiles and issue mma.sync.m16n8k8 instead.
+// Weight gradient: GEMM-K is the pixel dimension, so both NDHWC operands are MN-major, which wgmma does not accept from
+// shared memory for TF32.  A pre-pass copies the un-shifted operand channel-major in tile order (the K-major B operand);
+// the tap-shifted one stays channel-minor and reaches wgmma through registers (the register-A form), with the filter taps
+// folded into GEMM-M.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -31,7 +33,6 @@ namespace vp {
 constexpr int kMaxTaps = 128;
 constexpr int kMaxMaps = 8;
 constexpr int kMaxStagesFwd = 8;
-constexpr int kWgPix = 64;  // pixels (GEMM-K) per wgrad pipeline stage
 
 struct Tap {
   int8_t map, cd, ch, cw;
@@ -40,7 +41,7 @@ struct Tap {
 
 struct alignas(64) IgemmArgs {
   CUtensorMap amap[kMaxMaps];  // shifted operand, one map per stride parity
-  CUtensorMap bmap;            // fwd: packed weights (2-D);  wgrad: the un-shifted operand (5-D)
+  CUtensorMap bmap;            // packed weights (2-D)
   int32_t tiles_w, tiles_h, tiles_d, tiles_n;
   int32_t bw, bh, bd, bn;
   int32_t kc, n_pad, bn_tile;
@@ -58,9 +59,7 @@ struct alignas(64) IgemmArgs {
   const float* aux_y;    // optional: activation OUTPUT with the layout of `out`; result is multiplied by act'(aux_y)
   const float* aux_add;  // optional addend (same layout), added before the multiplication
   int32_t aux_act;
-  // wgrad only
-  int32_t rows_from_shifted, m_tiles, n_tiles, kpad;
-  int32_t num_taps, rows_valid, stages;
+  int32_t stages;
   int32_t k_tail;        // MMAs (K = 8 channels each) that hold real channels in the LAST k-chunk of a tap (1..4)
   Tap taps[kMaxTaps];
 };
@@ -231,33 +230,61 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
 }
 
 // ------------------------------------------------------------------------------------------------
-// wgrad kernel: one CTA = (128 dy-channels x up-to-128 x-channels) x ONE filter tap x a range of 64-pixel boxes.
-// Per box, warp 0 loads the dy and x tiles (<= 4 + 4 boxes of 64 pixels x 32 channels, 128B-swizzled); the shifted
-// operand (x for a conv, dy for a transposed conv) is read at the tap's coordinate shift.  Warps 1..8 own 16 dy channels
-// each and accumulate their 16 x (32 nb) slice of dW over the CTA's whole pixel range in registers.  Every dW element has
-// one owner per pixel-range split, which adds its sum without atomics: into dW itself when there is one split, otherwise
-// into the split's own zero-filled scratch plane (so_n floats apart), which reduce_parts then adds to dW in split order.
+// Weight gradient.  Of the two operands one is read at a per-tap shift ("shifted": x of a conv, which reads x at
+// s*o + r - p; dy of a transposed conv, which writes dy there) and the other without one ("plain": dy of a conv, x of a
+// transposed conv); the sum runs over the plain operand's pixels o, and tap r reads the shifted operand at position o + c_r
+// of its stride-parity lattice q_r (q_r = (r - p) mod s, c_r = floor((r - p) / s)).
+// wgrad_xt_kernel copies the plain operand once per call into scratch as T[c][pixel], channel-major, pixels in the main
+// kernel's 64-pixel tile order and zero outside the lattice: a K-major wgmma B operand (N = plain channels, K = pixels),
+// fetched with 32-pixel x BN-channel TMA boxes (channels past the view are TMA zero fill).  The filter taps are folded into
+// GEMM-M: a CTA owns four 32-row blocks, each a (tap, 32-channel chunk of the shifted operand) pair whose rows are a 5-D
+// TMA box of the tap's parity lattice at the tap's shift (channel-minor, 128B swizzle, zero fill = the padding), so one B
+// tile per 64 pixels serves all of a CTA's taps.  Each thread loads its A fragments from the box with lds and issues
+// wgmma.m64nBNk8 in the register-A form.  The products of a dW element are summed in pixel order, 8 pixels per MMA, over
+// the tiles of its pixel-range split.
 // ------------------------------------------------------------------------------------------------
-constexpr int kWgMaxStages = 4;
-constexpr int kWgThreads = 288;
-__global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid_constant__ IgemmArgs a) {
+constexpr int kWgTile = 64;        // pixels (GEMM-K) per pipeline stage
+constexpr int kWgBlocks = 4;       // 32-row (tap, channel chunk) blocks per CTA: two per consumer warpgroup
+constexpr int kWgMaxStages = 6;
+constexpr int kWgThreads = 384;
+
+struct alignas(64) WgradArgs {
+  CUtensorMap amap[kMaxMaps];      // shifted operand, one map per stride parity; box: 32 channels x the pixel box
+  CUtensorMap tmap;                // plain operand transposed, 2-D [channel][pixel]
+  int32_t bw, bh, bd, bn;          // pixel box, w fastest, bw * bh * bd * bn = kWgTile
+  int32_t tiles_w, tiles_h, tiles_d, tiles_n;
+  int32_t num_taps, chunks, n_tiles, splits, stages;
+  int32_t rows_valid, cols_valid;  // channels of the shifted (GEMM-M) and plain (GEMM-N) operands
+  int32_t rows_are_ci;             // 1: GEMM-M is x's channels (conv), 0: dy's channels (transposed conv)
+  int32_t n_pad, kpad;
+  float* out;
+  long long so_n;
+  Tap taps[kMaxTaps];
+};
+
+// Row rho (0..31) of a row block holds channel 4 (rho / 8) + (rho % 4) + 16 ((rho % 8) / 4): lanes g = 0..7 of one
+// fragment load then read channels {x..x+3, x+16..x+19}, whose 16-byte chunks under the 128B swizzle fall on 32 different
+// banks for the four pixel rows t = 0..3 (a contiguous 8 channels would be a 2-way conflict).
+__device__ __forceinline__ int wg_row_channel(int rho) { return 4 * (rho >> 3) + (rho & 3) + 16 * ((rho >> 2) & 1); }
+
+template <int BN>
+__global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid_constant__ WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ uint64_t full_bar[kWgMaxStages], empty_bar[kWgMaxStages];
-  constexpr uint32_t kSub = kWgPix * 128;  // bytes of one 64-pixel x 32-channel box
+  constexpr uint32_t kBox = kWgTile * 128;                  // one row block: 64 pixels x 32 channels
+  constexpr uint32_t kTHalf = BN * 128;                     // 32 pixels of the B tile: BN channel rows of 128 B
+  constexpr uint32_t kStage = kWgBlocks * kBox + 2 * kTHalf;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mtile = blockIdx.x % a.m_tiles, ntile = blockIdx.x / a.m_tiles;
-  const int m0 = mtile * 128;                                   // dy channel (row) origin
-  const int c0 = ntile * 128;                                   // x channel (col) origin
-  const int nb = min(4, a.kc - ntile * 4);                      // 32-channel boxes of x in this tile
-  const int na = min(4, (a.rows_valid - m0 + 31) / 32);         // 32-channel boxes of dy that hold real channels
-  const Tap tp = a.taps[blockIdx.y];
-  const uint32_t stage_bytes = static_cast<uint32_t>(na + nb) * kSub;
+  const int wg = threadIdx.x >> 7;
+  const int ntile = blockIdx.x % a.n_tiles;
+  const int blk0 = (blockIdx.x / a.n_tiles) * kWgBlocks;
+  const int nblk = min(kWgBlocks, a.num_taps * a.chunks - blk0);
+  const int c0 = ntile * BN;
   const int total = a.tiles_w * a.tiles_h * a.tiles_d * a.tiles_n;
-  const int it0 = static_cast<int>(static_cast<long long>(total) * blockIdx.z / a.splits);
-  const int it1 = static_cast<int>(static_cast<long long>(total) * (blockIdx.z + 1) / a.splits);
-  if (it1 <= it0 || na <= 0) return;
+  const int it0 = static_cast<int>(static_cast<long long>(total) * blockIdx.y / a.splits);
+  const int it1 = static_cast<int>(static_cast<long long>(total) * (blockIdx.y + 1) / a.splits);
+  if (it1 <= it0) return;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < a.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
@@ -265,100 +292,133 @@ __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid
   }
   __syncthreads();
 
+  const uint32_t smem0 = smem_u32(smem);
   const uint32_t full0 = smem_u32(&full_bar[0]), empty0 = smem_u32(&empty_bar[0]);
   const uint32_t ring_end = static_cast<uint32_t>(a.stages) * 8u;
-  const uint32_t smem0 = smem_u32(smem);
-  if (warp == 0) {
-    if (lane == 0) {
-      // dy boxes first, then the x boxes; the plain operand (bmap) is un-shifted, the other one is read at the tap's shift
-      const bool dy_shifted = a.rows_from_shifted != 0;
-      const CUtensorMap* map = &a.amap[tp.map];
-      int mt = it0;
-      int tw = mt % a.tiles_w; mt /= a.tiles_w;
-      int th = mt % a.tiles_h; mt /= a.tiles_h;
-      int td = mt % a.tiles_d;
-      int tn = mt / a.tiles_d;
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
+      int rem = it0;
+      int tw = rem % a.tiles_w; rem /= a.tiles_w;
+      int th = rem % a.tiles_h; rem /= a.tiles_h;
+      int td = rem % a.tiles_d;
+      int tn = rem / a.tiles_d;
+      const uint32_t stage_tx = static_cast<uint32_t>(nblk) * kBox + 2 * kTHalf;
       uint32_t s_off = 0, b_off = 0, ph = 0;
 #pragma unroll 1
       for (int it = it0; it < it1; ++it) {
         const int x0 = tw * a.bw, y0 = th * a.bh, d0 = td * a.bd, s0 = tn * a.bn;
         mbar_wait_addr(empty0 + b_off, ph ^ 1);
-        const uint32_t fb = full0 + b_off;
-        uint32_t dst = smem0 + s_off;
-        mbar_expect_tx_addr(fb, stage_bytes);
-        for (int i = 0; i < na; ++i, dst += kSub) {
-          if (dy_shifted) tma_load_5d_addr(dst, map, fb, m0 + 32 * i, x0 + tp.cw, y0 + tp.ch, d0 + tp.cd, s0);
-          else tma_load_5d_addr(dst, &a.bmap, fb, m0 + 32 * i, x0, y0, d0, s0);
+        const uint32_t fb = full0 + b_off, dst = smem0 + s_off;
+        mbar_expect_tx_addr(fb, stage_tx);
+        for (int j = 0; j < nblk; ++j) {
+          const int b = blk0 + j;
+          const Tap tp = a.taps[b / a.chunks];
+          tma_load_5d_addr(dst + j * kBox, &a.amap[tp.map], fb, 32 * (b % a.chunks), x0 + tp.cw, y0 + tp.ch, d0 + tp.cd, s0);
         }
-        for (int i = 0; i < nb; ++i, dst += kSub) {
-          if (dy_shifted) tma_load_5d_addr(dst, &a.bmap, fb, c0 + 32 * i, x0, y0, d0, s0);
-          else tma_load_5d_addr(dst, map, fb, c0 + 32 * i, x0 + tp.cw, y0 + tp.ch, d0 + tp.cd, s0);
-        }
+        tma_load_2d_addr(dst + kWgBlocks * kBox, &a.tmap, fb, it * kWgTile, c0);
+        tma_load_2d_addr(dst + kWgBlocks * kBox + kTHalf, &a.tmap, fb, it * kWgTile + 32, c0);
         if (++tw == a.tiles_w) { tw = 0; if (++th == a.tiles_h) { th = 0; if (++td == a.tiles_d) { td = 0; ++tn; } } }
-        s_off += stage_bytes; b_off += 8;
+        s_off += kStage; b_off += 8;
         if (b_off == ring_end) { s_off = 0; b_off = 0; ph ^= 1; }
       }
     }
     return;
   }
 
-  // ---- MMA warps: warp w (1..8) owns dy channels m0 + 16 (w - 1) .. + 15, all 32 nb x channels
-  const int cw = warp - 1;
+  // ---- consumers: warpgroup h owns row blocks 2h, 2h + 1; warp w of it rows 16 (w % 2) .. + 15 of block 2h + w / 2
+  const int h = wg - 1, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const bool active = 16 * cw < 32 * na;
-  const uint32_t a_box = static_cast<uint32_t>(cw >> 1) * kSub;
-  const int a_c = (cw & 1) * 16 + g;
-  const int nfr = 4 * nb;
-  float acc[16][4];
+  const int j = 2 * h + (w >> 1);
+  const bool live = j < nblk;
+  const int c_lo = wg_row_channel(16 * (w & 1) + g), c_hi = wg_row_channel(16 * (w & 1) + 8 + g);
+  const uint64_t bd_base = make_wgmma_desc(smem0 + kWgBlocks * kBox, 16, 1024, kWgmmaSwizzle128B);
+  float acc[BN / 2];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   uint32_t s_off = 0, b_off = 0, ph = 0;
 #pragma unroll 1
   for (int it = it0; it < it1; ++it) {
     mbar_wait_addr(full0 + b_off, ph);
-    if (active) {
-      const uint32_t abase = smem0 + s_off + a_box;
-      const uint32_t xbase = smem0 + s_off + static_cast<uint32_t>(na) * kSub;
-#pragma unroll 2
-      for (int k0 = 0; k0 < kWgPix; k0 += 8) {
-        uint32_t af[4];
-        af[0] = lds_u32(abase + sw128_offset(k0 + t, a_c));
-        af[1] = lds_u32(abase + sw128_offset(k0 + t, a_c + 8));
-        af[2] = lds_u32(abase + sw128_offset(k0 + t + 4, a_c));
-        af[3] = lds_u32(abase + sw128_offset(k0 + t + 4, a_c + 8));
+    uint32_t af[8][4];
+    const uint32_t ab = smem0 + s_off + static_cast<uint32_t>(j) * kBox;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (j < nfr) {
-            const uint32_t xb = xbase + static_cast<uint32_t>(j >> 2) * kSub;
-            const int c = (j & 3) * 8 + g;
-            uint32_t bf[2];
-            bf[0] = lds_u32(xb + sw128_offset(k0 + t, c));
-            bf[1] = lds_u32(xb + sw128_offset(k0 + t + 4, c));
-            mma_tf32_16x8x8(acc[j], af, bf);
-          }
-        }
-      }
+    for (int ks = 0; ks < 8; ++ks) {
+      const int k = 8 * ks + t;
+      af[ks][0] = live ? lds_u32(ab + sw128_offset(k, c_lo)) : 0u;
+      af[ks][1] = live ? lds_u32(ab + sw128_offset(k, c_hi)) : 0u;
+      af[ks][2] = live ? lds_u32(ab + sw128_offset(k + 4, c_lo)) : 0u;
+      af[ks][3] = live ? lds_u32(ab + sw128_offset(k + 4, c_hi)) : 0u;
     }
+    const uint64_t bd = bd_base + (s_off >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks)
+      WgmmaRS<BN>::mma(acc, af[ks], bd + (ks < 4 ? 2 * ks : kTHalf / 16 + 2 * (ks - 4)));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
     __syncwarp();
     if (lane == 0) mbar_arrive_addr(empty0 + b_off);
-    s_off += stage_bytes; b_off += 8;
+    s_off += kStage; b_off += 8;
     if (b_off == ring_end) { s_off = 0; b_off = 0; ph ^= 1; }
   }
-  if (!active) return;
-  const int row_end = min(a.n_pad, a.rows_valid);
+  if (!live) return;
+  // every dW element has one owner per pixel-range split, which adds its sum without atomics: into dW itself when there is
+  // one split, otherwise into the split's own zero-filled scratch plane, which reduce_parts adds to dW in split order
+  const int b = blk0 + j;
+  const Tap tp = a.taps[b / a.chunks];
+  float* plane = a.out + blockIdx.y * a.so_n + static_cast<long long>(tp.wslot) * a.n_pad * a.kpad;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    const int row = m0 + 16 * cw + g + 8 * r;
-    if (row >= row_end) continue;
-    float* orow = a.out + blockIdx.z * a.so_n + (static_cast<long long>(tp.wslot) * a.n_pad + row) * a.kpad + c0 + 2 * t;
+    const int row = 32 * (b % a.chunks) + (r ? c_hi : c_lo);
+    if (row >= a.rows_valid) continue;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      if (j < nfr) {
-        float2* o = reinterpret_cast<float2*>(orow + 8 * j);
-        const float2 e = *o;
-        *o = make_float2(e.x + acc[j][2 * r], e.y + acc[j][2 * r + 1]);
+    for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = c0 + 8 * i + 2 * t + e;
+        if (col >= a.cols_valid) continue;
+        // dW is [co][ci]: GEMM rows are x channels (ci) for a conv and dy channels (co) for a transposed conv
+        float* o = a.rows_are_ci ? plane + static_cast<long long>(col) * a.kpad + row : plane + static_cast<long long>(row) * a.kpad + col;
+        *o += acc[4 * i + 2 * r + e];
       }
     }
+  }
+}
+
+// T[c][tile * 64 + k] = the plain operand at pixel k of tile `tile` (0 outside the tensor).  One block transposes one tile
+// x 32 channels through shared memory: reads run along channels, writes along pixels.
+struct TransposeArgs {
+  const float* src;
+  long long cstride;
+  int32_t n, d, h, w, c;
+  int32_t bw, bh, bd, bn;
+  int32_t tiles_w, tiles_h, tiles_d;
+  float* dst;
+  long long p_pad;                 // pixels per channel row of T
+};
+
+__global__ void __launch_bounds__(256) wgrad_transpose_kernel(const __grid_constant__ TransposeArgs a) {
+  __shared__ float tile_s[32][kWgTile + 1];
+  const int tile = blockIdx.x;
+  const int tw = tile % a.tiles_w, th = (tile / a.tiles_w) % a.tiles_h, td = (tile / (a.tiles_w * a.tiles_h)) % a.tiles_d;
+  const int tn = tile / (a.tiles_w * a.tiles_h * a.tiles_d);
+  const int c0 = blockIdx.y * 32;
+  for (int e = threadIdx.x; e < kWgTile * 32; e += blockDim.x) {
+    const int k = e >> 5, c = e & 31;
+    const int pw = tw * a.bw + k % a.bw, ph = th * a.bh + (k / a.bw) % a.bh;
+    const int pd = td * a.bd + (k / (a.bw * a.bh)) % a.bd, pn = tn * a.bn + k / (a.bw * a.bh * a.bd);
+    float v = 0.f;
+    if (pw < a.w && ph < a.h && pd < a.d && pn < a.n && c0 + c < a.c) {
+      const long long pix = ((static_cast<long long>(pn) * a.d + pd) * a.h + ph) * a.w + pw;
+      v = __ldg(a.src + pix * a.cstride + c0 + c);
+    }
+    tile_s[c][k] = v;
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < kWgTile * 32; e += blockDim.x) {
+    const int c = e / kWgTile, k = e % kWgTile;
+    if (c0 + c < a.c) a.dst[static_cast<long long>(c0 + c) * a.p_pad + static_cast<long long>(tile) * kWgTile + k] = tile_s[c][k];
   }
 }
 
@@ -402,30 +462,40 @@ static int check_tensor(const vp_tensor* t, const char* what) {
   return 0;
 }
 
+// Taps of a (non-transposed) convolution in weight-slot order: tap r reads the input at s * o + r - p, i.e. at lattice
+// position o + c_r of the stride-parity sub-lattice q_r (map = q_r, (cd, ch, cw) = c_r).  Returns the count, -1 on error.
+static int conv_taps(const vp_conv_geom* g, Tap* taps) {
+  const int K = g->kd * g->kh * g->kw;
+  if (K > kMaxTaps) return set_error("too many filter taps (%d)", K);
+  if (g->sd * g->sh * g->sw > kMaxMaps) return set_error("stride product too large");
+  int n = 0;
+  for (int rd = 0; rd < g->kd; ++rd)
+    for (int rh = 0; rh < g->kh; ++rh)
+      for (int rw = 0; rw < g->kw; ++rw) {
+        Tap& t = taps[n++];
+        const int qd = pos_mod(rd - g->pd, g->sd), qh = pos_mod(rh - g->ph, g->sh), qw = pos_mod(rw - g->pw, g->sw);
+        t.map = static_cast<int8_t>((qd * g->sh + qh) * g->sw + qw);
+        t.cd = static_cast<int8_t>(floor_div(rd - g->pd, g->sd));
+        t.ch = static_cast<int8_t>(floor_div(rh - g->ph, g->sh));
+        t.cw = static_cast<int8_t>(floor_div(rw - g->pw, g->sw));
+        t.wslot = (rd * g->kh + rh) * g->kw + rw;
+      }
+  return n;
+}
+
 // Fills taps / phases / output strides of the geometry; `lat` (w,h,d,n) is divided by the stride for transposed convs.
 static int build_taps(IgemmArgs& A, const vp_conv_geom* g, int lat[4]) {
   int ntaps = 0;
-  const int K = g->kd * g->kh * g->kw;
-  if (K > kMaxTaps) return set_error("too many filter taps (%d)", K);
   if (!g->transposed) {
-    if (g->sd * g->sh * g->sw > kMaxMaps) return set_error("stride product too large");
+    ntaps = conv_taps(g, A.taps);
+    if (ntaps < 0) return -1;
     A.num_phases = 1;
     A.phase_begin[0] = 0;
     A.os_d = A.os_h = A.os_w = 1;
     std::memset(A.phase_ooff, 0, sizeof(A.phase_ooff));
-    for (int rd = 0; rd < g->kd; ++rd)
-      for (int rh = 0; rh < g->kh; ++rh)
-        for (int rw = 0; rw < g->kw; ++rw) {
-          Tap& t = A.taps[ntaps++];
-          const int qd = pos_mod(rd - g->pd, g->sd), qh = pos_mod(rh - g->ph, g->sh), qw = pos_mod(rw - g->pw, g->sw);
-          t.map = static_cast<int8_t>((qd * g->sh + qh) * g->sw + qw);
-          t.cd = static_cast<int8_t>(floor_div(rd - g->pd, g->sd));
-          t.ch = static_cast<int8_t>(floor_div(rh - g->ph, g->sh));
-          t.cw = static_cast<int8_t>(floor_div(rw - g->pw, g->sw));
-          t.wslot = (rd * g->kh + rh) * g->kw + rw;
-        }
     A.phase_begin[1] = ntaps;
   } else {
+    if (g->kd * g->kh * g->kw > kMaxTaps) return set_error("too many filter taps (%d)", g->kd * g->kh * g->kw);
     const int P = g->sd * g->sh * g->sw;
     if (P > 8) return set_error("stride product too large");
     A.num_phases = P;
@@ -596,51 +666,110 @@ extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_c
   if (check_tensor(x, "vp_conv_wgrad(x)") || check_tensor(dy, "vp_conv_wgrad(dy)")) return -1;
   if (!g || !dwpacked) return set_error("vp_conv_wgrad: null argument");
   if (n_pad % 16 || dy->c > n_pad || kc * 32 < x->c) return set_error("vp_conv_wgrad: bad n_pad / kc");
-  static thread_local IgemmArgs A;
+  static thread_local WgradArgs A;
   std::memset(&A, 0, sizeof(A));
-  // conv:  dW[r] += sum_o dy[o]^T x[s*o+r-p]   (x shifted, lattice = dy)
-  // tconv: dW[r] += sum_o dy[s*o+r-p]^T x[o]   (dy shifted, lattice = x); as a gather this is a
-  //        plain (non-transposed) strided access pattern, so build the geometry with transposed=0.
+  // conv:  dW[r] += sum_o x[s*o+r-p]^T dy[o]   (x shifted, lattice = dy)
+  // tconv: dW[r] += sum_o dy[s*o+r-p]^T x[o]   (dy shifted, lattice = x); as a gather this is a plain (non-transposed)
+  //        strided access pattern, so the taps are those of the geometry with transposed = 0.
   vp_conv_geom gg = *g;
   gg.transposed = 0;
   const vp_tensor* shifted = g->transposed ? dy : x;
   const vp_tensor* plain = g->transposed ? x : dy;
-  const int lat[4] = {plain->w, plain->h, plain->d, plain->n};
-  if (build_geometry(A, &gg, shifted, kWgPix, lat)) return -1;
+  const int ntaps = conv_taps(&gg, A.taps);
+  if (ntaps < 0) return -1;
+  A.num_taps = ntaps;
+  int rem = kWgTile;
+  A.bw = std::min(floor_pow2(plain->w), rem); rem /= A.bw;
+  A.bh = std::min(floor_pow2(plain->h), rem); rem /= A.bh;
+  A.bd = std::min(floor_pow2(plain->d), rem); rem /= A.bd;
+  A.bn = rem;
+  A.tiles_w = ceil_div(plain->w, A.bw); A.tiles_h = ceil_div(plain->h, A.bh);
+  A.tiles_d = ceil_div(plain->d, A.bd); A.tiles_n = ceil_div(plain->n, A.bn);
+  const long long total = static_cast<long long>(A.tiles_w) * A.tiles_h * A.tiles_d * A.tiles_n;
+  if (total * kWgTile > (1LL << 31) - 1) return set_error("vp_conv_wgrad: too many pixels");
   const int box[4] = {A.bw, A.bh, A.bd, A.bn};
-  if (make_act_map(&A.bmap, plain, 0, 0, 0, 1, 1, 1, box)) return -1;
-  A.rows_from_shifted = g->transposed ? 1 : 0;
-  A.kc = kc; A.n_pad = n_pad; A.kpad = kc * 32;
-  A.rows_valid = dy->c;
-  A.m_tiles = ceil_div(std::min(n_pad, ceil_div(dy->c, 32) * 32), 128);
-  A.n_tiles = ceil_div(kc, 4);
-  A.num_taps = A.phase_begin[1];
-  const int na_max = std::min(4, ceil_div(dy->c, 32)), nb_max = std::min(4, kc);
-  const size_t stage_bytes = static_cast<size_t>(na_max + nb_max) * kWgPix * 128;
+  for (int qd = 0; qd < g->sd; ++qd)
+    for (int qh = 0; qh < g->sh; ++qh)
+      for (int qw = 0; qw < g->sw; ++qw)
+        if (make_act_map(&A.amap[(qd * g->sh + qh) * g->sw + qw], shifted, qd, qh, qw, g->sd, g->sh, g->sw, box)) return -1;
+  A.chunks = ceil_div(shifted->c, 32);
+  A.rows_valid = shifted->c; A.cols_valid = plain->c;
+  A.rows_are_ci = g->transposed ? 0 : 1;
+  A.n_pad = n_pad; A.kpad = kc * 32;
+  const int m_tiles = ceil_div(ntaps * A.chunks, kWgBlocks);
+  // N tile (GEMM-N = plain channels): the wgmma N whose tiles cover them with the fewest padded columns (ties: the wider)
+  int bn_tile = 32;
+  {
+    int best = 1 << 30;
+    for (int bn : {136, 128, 72, 64, 32}) {
+      const int cols = ceil_div(plain->c, bn) * bn;
+      if (cols < best) { best = cols; bn_tile = bn; }
+    }
+  }
+  A.n_tiles = ceil_div(plain->c, bn_tile);
+  const size_t stage_bytes = static_cast<size_t>(kWgBlocks) * kWgTile * 128 + 2 * static_cast<size_t>(bn_tile) * 128;
   const size_t smem_max = 227 * 1024 - 2048;
   A.stages = static_cast<int>(std::min<size_t>(kWgMaxStages, (smem_max - 1024) / stage_bytes));
-  const int total = A.tiles_w * A.tiles_h * A.tiles_d * A.tiles_n;
-  const int ctas = A.m_tiles * A.n_tiles * A.num_taps;
-  if (split_k <= 0) split_k = std::max(1, (2 * device_sms()) / ctas);  // auto: at most two full waves (never a third partial wave)
-  A.splits = std::max(1, std::min(split_k, std::max(1, total / 4)));
-  const long long plane = static_cast<long long>(A.num_taps) * n_pad * A.kpad;
-  float* ws = nullptr;
-  if (A.splits > 1 && scratch_zeroed(&ws, A.splits * plane, stream)) return -1;
-  A.out = A.splits > 1 ? ws : dwpacked;
-  A.so_n = plane;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(igemm_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
-      return set_error("cudaFuncSetAttribute(igemm_wgrad_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
-    attr_set = true;
+  // The pixel range is split by a rule of the layer's shape alone -- two waves of (taps x 128-row dy tiles x 128-column x
+  // tiles) CTAs, at least four tiles per split -- not of the kernel's tiling, so the grouping of every dW sum (and with
+  // it the fp32 result) depends only on the layer.
+  if (split_k <= 0) {
+    const int ctas = ntaps * ceil_div(std::min(n_pad, ceil_div(dy->c, 32) * 32), 128) * ceil_div(kc, 4);
+    split_k = std::max(1, (2 * device_sms()) / ctas);
   }
-  const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
-  dim3 grid(A.m_tiles * A.n_tiles, A.num_taps, A.splits);
-  igemm_wgrad_kernel<<<grid, kWgThreads, smem, static_cast<cudaStream_t>(stream)>>>(A);
-  int rc = check_launch("igemm_wgrad_kernel");
+  A.splits = static_cast<int>(std::max<long long>(1, std::min<long long>(split_k, std::max<long long>(1, total / 4))));
+
+  TransposeArgs T;
+  std::memset(&T, 0, sizeof(T));
+  T.src = plain->ptr; T.cstride = plain->cstride;
+  T.n = plain->n; T.d = plain->d; T.h = plain->h; T.w = plain->w; T.c = plain->c;
+  T.bw = A.bw; T.bh = A.bh; T.bd = A.bd; T.bn = A.bn;
+  T.tiles_w = A.tiles_w; T.tiles_h = A.tiles_h; T.tiles_d = A.tiles_d;
+  T.p_pad = total * kWgTile;
+  float* tbuf = nullptr;
+  if (scratch_alloc(&tbuf, static_cast<long long>(plain->c) * T.p_pad, stream)) return -1;
+  T.dst = tbuf;
+  {
+    EncodeTiledFn enc = get_encode();
+    if (!enc) { scratch_free(tbuf, stream); return set_error("cuTensorMapEncodeTiled entry point not found"); }
+    cuuint64_t dims[2] = {static_cast<cuuint64_t>(T.p_pad), static_cast<cuuint64_t>(plain->c)};
+    cuuint64_t strides[1] = {static_cast<cuuint64_t>(T.p_pad) * 4};
+    cuuint32_t boxd[2] = {32, static_cast<cuuint32_t>(bn_tile)};
+    cuuint32_t es[2] = {1, 1};
+    CUresult r = enc(&A.tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, tbuf, dims, strides, boxd, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { scratch_free(tbuf, stream); return set_error("cuTensorMapEncodeTiled(transposed operand) failed with %d", static_cast<int>(r)); }
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  wgrad_transpose_kernel<<<dim3(static_cast<unsigned>(total), ceil_div(plain->c, 32)), 256, 0, st>>>(T);
+  int rc = check_launch("wgrad_transpose_kernel");
+  const long long plane = static_cast<long long>(ntaps) * n_pad * A.kpad;
+  float* ws = nullptr;
+  if (!rc && A.splits > 1) rc = scratch_zeroed(&ws, A.splits * plane, stream);
+  if (!rc) {
+    A.out = A.splits > 1 ? ws : dwpacked;
+    A.so_n = plane;
+    typedef void (*WgKernel)(const WgradArgs);
+    static const WgKernel kernels[5] = {igemm_wgrad_kernel<32>, igemm_wgrad_kernel<64>, igemm_wgrad_kernel<72>,
+                                        igemm_wgrad_kernel<128>, igemm_wgrad_kernel<136>};
+    static bool attr_set = false;
+    if (!attr_set) {
+      for (WgKernel k : kernels)
+        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
+          rc = set_error("cudaFuncSetAttribute(igemm_wgrad_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
+      attr_set = rc == 0;
+    }
+    if (!rc) {
+      const WgKernel kernel = kernels[bn_tile == 32 ? 0 : bn_tile == 64 ? 1 : bn_tile == 72 ? 2 : bn_tile == 128 ? 3 : 4];
+      const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
+      kernel<<<dim3(m_tiles * A.n_tiles, A.splits), kWgThreads, smem, st>>>(A);
+      rc = check_launch("igemm_wgrad_kernel");
+    }
+  }
   if (ws) {
     if (!rc) rc = reduce_parts(ws, A.splits, plane, dwpacked, stream);
     scratch_free(ws, stream);
   }
+  scratch_free(tbuf, stream);
   return rc;
 }

@@ -246,6 +246,16 @@ int vp_pix_distrib_fwd(const int32_t* sel, const float* pix_gt, const float* pix
                        int transformed_cstride, int slot_stride, int n, int h, int w, int d, int kh, int kw, int nk,
                        vp_stream_t stream);
 
+/* Robot-state recurrence of the action-conditioned cell (savp_model.py:411-412, 655-658), all s steps of n rows in one
+ * launch, forward only (no loss reads the predicted states).  For t < s and row r < n:
+ *   state_t     = sel[t*n + r] ? states[(t*n + r) * states_stride + j] : gen_state_{t-1}   (gen_state_{-1} = 0)
+ *   zvec[(t*n + r) * zvec_stride + a + j] = state_t[j]                                   j < sd
+ *   gen_states[(t*n + r) * sd + j] = bias[j] + sum_{i < a + sd} x[i] * kernel[i * sd + j],  x = zvec row [0, a + sd)
+ * The actions are read from zvec channels [0, a), where the caller staged them; only channels [a, a + sd) of zvec are
+ * written.  Each sum is added in increasing i without atomics: identical inputs give identical bits. */
+int vp_state_pred_fwd(const int32_t* sel, const float* states, int states_stride, const float* kernel, const float* bias,
+                      float* zvec, int zvec_stride, float* gen_states, int s, int n, int a, int sd, vp_stream_t stream);
+
 /* ---- losses (losses.py:6-67): out[0] += value; optional gradient = grad_scale * d value / d pred -------- */
 int vp_pixel_loss(const float* pred, int pred_cstride, const float* target, int target_cstride, float* dpred,
                   int dpred_cstride, long long rows, int c, int mode /*bit 0: 0 = L1, 1 = L2; bit 1: dpred += instead of =*/, long long mean_count,

@@ -12,7 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 LIB_PATH = os.path.join(HERE, 'libvp_b200.so')
-SOURCES = ['api.cu', 'igemm.cu', 'pack.cu', 'elementwise.cu', 'backward.cu', 'discrim.cu', 'planes.cu', 'd0_layer.cu', 'pixdistrib.cu']
+SOURCES = ['api.cu', 'igemm.cu', 'pack.cu', 'elementwise.cu', 'backward.cu', 'discrim.cu', 'planes.cu', 'd0_layer.cu', 'pixdistrib.cu',
+           'statepred.cu']
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17',
                      '-Xcompiler', '-fPIC', '--use_fast_math', '-Xptxas', '-v',

@@ -5,7 +5,7 @@ train on are read on the host without TensorFlow (`video_datasets.py`, `tfrecord
 `bair`) and KTH (`kth`); the other registered names (JPEG-encoded or unused by any shipped config) raise
 NotImplementedError.  `synthetic` is the dataset the hot path is measured on:
 seeded videos of the shape the reference datasets deliver (`images` [B,T,H,W,C] f32 in [0,1], optional `actions`
-[B,T-1,A]; base_dataset.py:189), generated on the host, so `scripts/train.py --dataset synthetic` and
+[B,T-1,A] and, with use_state, `states` [B,T,state_dim]; base_dataset.py:189), generated on the host, so `scripts/train.py --dataset synthetic` and
 `scripts/generate.py --dataset synthetic` run end to end without any input files."""
 from __future__ import annotations
 
@@ -39,7 +39,7 @@ class SyntheticVideoDataset(object):
         # base_dataset.py:84-96 + the synthetic shape knobs (defaults: the BAIR action-free shape, 2 + 10 frames)
         return dict(crop_size=0, scale_size=0, context_frames=2, sequence_length=12, long_sequence_length=0, frame_skip=0,
                     time_shift=1, force_time_shift=False, shuffle_on_val=False, use_state=False,
-                    image_size=(64, 64), channels=3, action_dim=0, num_examples=256, smooth=True)
+                    image_size=(64, 64), channels=3, action_dim=0, state_dim=3, num_examples=256, smooth=True)
 
     def get_default_hparams(self):
         return HParams(**self.get_default_hparams_dict())
@@ -89,6 +89,8 @@ class SyntheticVideoDataset(object):
         batch = {'images': self._videos(batch_size)}
         if hp.action_dim:
             batch['actions'] = self._rng.standard_normal((batch_size, hp.sequence_length - 1, hp.action_dim)).astype(np.float32)
+        if hp.use_state:      # robot states, [B,T,state_dim] like BAIR's endeffector_pos (state_dim 3)
+            batch['states'] = self._rng.standard_normal((batch_size, hp.sequence_length, hp.state_dim)).astype(np.float32)
         return batch
 
 

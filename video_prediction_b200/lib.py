@@ -367,6 +367,13 @@ def pix_distrib_fwd(sel, pix_gt_addr, pix_first_addr, pix_cs, gen_prev_addr, ker
                                    C.c_void_p(tr_addr), tr_cs, slot_stride, n, h, w, d, kh, kw, nk, stream_ptr()))
 
 
+def state_pred_fwd(sel, states, states_stride, kernel, bias, zvec, zvec_stride, gen_states, s, n, a, sd):
+    """The robot-state recurrence of all s steps (vp_state_pred_fwd): writes the selected states into zvec channels
+    [a, a + sd) and the predictions into gen_states [s, n, sd]."""
+    check(lib().vp_state_pred_fwd(ptr(sel), ptr(states), states_stride, ptr(kernel), ptr(bias), ptr(zvec), zvec_stride,
+                                  ptr(gen_states), s, n, a, sd, stream_ptr()))
+
+
 # ---------------------------------------------------------------------------------- backward / losses / optimizer
 def _srcs(srcs):
     """srcs: list of (address:int, cstride:int) gradient sources to be summed."""

@@ -172,6 +172,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         self.params = None
         self.grads = None
         self.built = False
+        self.Sd = 0                      # robot-state dimensions, from build_graph's inputs
         self.world_size = 1
         self.rank = 0
         self.random_seed = 0
@@ -347,14 +348,18 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         nlayers = nk + 3
         specs[sc + '/masks/conv2d/kernel'] = ((3, 3, hp.ngf + nlayers * C, nlayers), 'kernel')
         specs[sc + '/masks/conv2d/bias'] = ((nlayers,), 'zeros')
+        if self.Sd:       # savp_model.py:655-658: the next robot state from [actions | state]
+            specs[sc + '/state_pred/dense/kernel'] = ((A + self.Sd, self.Sd), 'kernel')
+            specs[sc + '/state_pred/dense/bias'] = ((self.Sd,), 'zeros')
         return specs
 
     # ------------------------------------------------------------------ build
     def build_graph(self, inputs):
         """inputs: dict with 'images' [B,T,H,W,C] (torch / numpy, batch-major as in base_model.py:467)
-        and optionally 'actions' [B,T-1,A] and 'pix_distribs' [B,T,H,W,D] (D designated-pixel probability maps, moved
-        with the images: gen_pix_distribs / transformed_pix_distribs in `outputs`).  Allocates parameters (reference
-        initialisers) unless `set_params` was called, and all activation buffers."""
+        and optionally 'actions' [B,T-1,A], 'states' [B,T,Sd] (robot states: tile-concatenated into every convolution
+        input after the actions and predicted as gen_states) and 'pix_distribs' [B,T,H,W,D] (D designated-pixel
+        probability maps, moved with the images: gen_pix_distribs / transformed_pix_distribs in `outputs`).  Allocates
+        parameters (reference initialisers) unless `set_params` was called, and all activation buffers."""
         super(SAVPVideoPredictionModel, self).build_graph(inputs)
         if not torch.cuda.is_available():
             raise RuntimeError('video_prediction_b200 needs a CUDA device (sm_90a); there is no CPU fallback')
@@ -382,8 +387,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         self.B, self.T, self.H, self.W, self.C = B, hp.sequence_length, H, W, C
         self.A = int(inputs['actions'].shape[-1]) if 'actions' in inputs else 0
         self.D = self._pix_distribs_depth(inputs)
+        self.Sd = self._states_dim(inputs)
         self.S = self.T - 1
-        self.Zc = self.A + (hp.nz if hp.nz else 0)
+        self.Zc = self.A + self.Sd + (hp.nz if hp.nz else 0)     # tile-concat vector [actions | state | rnn_z]
         self.NB = 2 * B if hp.nz else B
         self.enc_specs, self.dec_specs = self.layer_specs(hp.ngf, H, W)
         total_stride = 2 ** len(self.enc_specs)
@@ -425,6 +431,18 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if int(pd.shape[4]) < 1:
             raise ValueError('pix_distribs need at least one designated pixel (D >= 1), got shape %s' % (tuple(pd.shape),))
         return int(pd.shape[4])
+
+    @staticmethod
+    def _states_dim(inputs):
+        """Sd of inputs['states'] [B,T,Sd] (0 without the key); the states must cover the images' frames."""
+        if 'states' not in inputs:
+            return 0
+        st, im = inputs['states'], inputs['images']
+        if len(st.shape) != 3 or tuple(st.shape[:2]) != tuple(im.shape[:2]):
+            raise ValueError('states must be [B, T, Sd] with B, T of the images %s, got %s' % (tuple(im.shape), tuple(st.shape)))
+        if int(st.shape[2]) < 1:
+            raise ValueError('states need at least one dimension (Sd >= 1), got shape %s' % (tuple(st.shape),))
+        return int(st.shape[2])
 
     def _alloc_params(self):
         """Flat fp32 buffers (one per optimizer: generator / discriminator, base_model.py:486-487) with
@@ -739,6 +757,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['tpix'] = self._z(S, NB, H, W, self.nlayers * Dp)
         if Zc:
             Bf['zvec'] = self._z(S, NB, _ceil4(Zc))
+        if self.Sd:
+            Bf['states'] = self._z(S, NB, self.Sd)     # ground-truth states of both unrolls
+            Bf['gstates'] = self._z(S, NB, self.Sd)    # predicted states (savp_model.py:655-658)
         if hp.nz:
             nz = hp.nz
             Bf['zs'] = self._z(S, NB, nz)             # zs fed to the two unrolls (posterior | prior)
@@ -757,6 +778,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         segs = [('a', C), ('b', C)] + ([('act', A)] if A else [])
         self.pair_spec = ConcatSpec(segs)
         Bf['pairs'] = self._z(S * B, H, W, self.pair_spec.cstride)
+        if A:
+            Bf['actions'] = self._z(S, B, A)             # the actions the posterior tile-concatenates (savp_model.py:24-26)
         self.enc_layers = []
         spec = self.pair_spec
         hh, ww = H, W
@@ -810,10 +833,19 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['x'][:, B:, :, :, :C] = x
         if self.A:
             act = torch.as_tensor(inputs['actions']).to(dev, torch.float32)[:, :S].permute(1, 0, 2)
-            self._actions = act.contiguous()
+            if hp.nz:        # a static buffer: the captured training step re-reads it on every replay
+                Bf['actions'].copy_(act)
             Bf['zvec'][:, :B, :self.A] = act
             if self.NB > B:
                 Bf['zvec'][:, B:, :self.A] = act
+        if self._states_dim(inputs) != self.Sd:
+            raise ValueError('the model was built %s states; the inputs must match'
+                             % ('with %d-dimensional' % self.Sd if self.Sd else 'without'))
+        if self.Sd:
+            st = torch.as_tensor(inputs['states']).to(dev, torch.float32)[:, :S].permute(1, 0, 2)
+            Bf['states'][:, :B] = st
+            if self.NB > B:
+                Bf['states'][:, B:] = st
         if self._pix_distribs_depth(inputs) != self.D:
             raise ValueError('the model was built %s pix_distribs; the inputs must match'
                              % ('with %d-channel' % self.D if self.D else 'without'))
@@ -942,7 +974,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             L.copy_channels(x[t].data_ptr(), 4, dst.data_ptr() + 4 * ps.off('a'), ps.cstride, B * H * W, 4)
             L.copy_channels(x[t + 1].data_ptr(), 4, dst.data_ptr() + 4 * ps.off('b'), ps.cstride, B * H * W, 4)
         if A:
-            L.broadcast_channels(self._actions, A, Bf['pairs'].data_ptr() + 4 * ps.off('act'), ps.cstride, S * B, H * W, A)
+            L.broadcast_channels(Bf['actions'], A, Bf['pairs'].data_ptr() + 4 * ps.off('act'), ps.cstride, S * B, H * W, A)
         cur = Bf['pairs']
         for i, el in enumerate(self.enc_layers):
             pre = Bf['epre%d' % i]
@@ -978,7 +1010,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         and every tile_concat of (actions, rnn_z) becomes one broadcast store per concat buffer."""
         hp = self.hparams
         Bf = self.Bf
-        S, NB, nz, A = self.S, self.NB, hp.nz, self.A
+        S, NB, nz, off = self.S, self.NB, hp.nz, self.A + self.Sd
         P = self.params
         b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
         Zp = _ceil4(self.Zc)
@@ -989,7 +1021,15 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             L.copy_channels(Bf['zh'][t].data_ptr(), nz, Bf['zcat'][t].data_ptr() + 4 * nz, 2 * nz, NB, nz)
             L.dense_fwd(Bf['zcat'][t], 2 * nz, P[b + '/kernel'], P[b + '/bias'], Bf['zgates'][t], 4 * nz, NB, 2 * nz, 4 * nz)
             L.lstm_cell_fwd(Bf['zgates'][t], Bf['zc'][t], Bf['zc'][t + 1], Bf['zh'][t + 1], NB, nz)
-            L.copy_channels(Bf['zh'][t + 1].data_ptr(), nz, Bf['zvec'][t].data_ptr() + 4 * A, Zp, NB, nz)
+            L.copy_channels(Bf['zh'][t + 1].data_ptr(), nz, Bf['zvec'][t].data_ptr() + 4 * off, Zp, NB, nz)
+
+    def _state_pred_forward(self):
+        """Robot states (savp_model.py:411-412, 655-658): like rnn_z independent of the images, so one launch runs the
+        recurrence of every step and row before the tile-concats; it reads the scheduled-sampling mask `sel` of this step."""
+        Bf, P = self.Bf, self.params
+        sc = 'generator/rnn/savp_cell/state_pred/dense'
+        L.state_pred_fwd(Bf['sel'], Bf['states'], self.Sd, P[sc + '/kernel'], P[sc + '/bias'], Bf['zvec'], _ceil4(self.Zc),
+                         Bf['gstates'], self.S, self.NB, self.A, self.Sd)
 
     def _broadcast_z(self):
         if not self.Zc:
@@ -1124,6 +1164,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if hp.nz:
             self._posterior_forward()
             self._rnn_z_forward()
+        if self.Sd:
+            self._state_pred_forward()
         self._broadcast_z()
         for d in self.gl:
             if d['use']:
@@ -1227,6 +1269,12 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             out['gen_images'] = gen.permute(1, 0, 2, 3, 4)
             out['transformed_images'] = tr.permute(1, 0, 2, 3, 4, 5)
             out['masks'] = masks.permute(1, 0, 2, 3, 4, 5)
+        if self.Sd:
+            gst = Bf['gstates'].permute(1, 0, 2)                                                   # [NB,S,Sd]
+            if self.hparams.nz:
+                out['gen_states_enc'] = gst[:B]
+                gst = gst[B:]
+            out['gen_states'] = gst
         if self.D:
             D, S, NB, H, W = self.D, self.S, self.NB, self.H, self.W
             gpix = Bf['gpix'][..., :D]                                                             # [S,NB,H,W,D]

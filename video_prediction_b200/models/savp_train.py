@@ -477,12 +477,13 @@ class TrainMixin(object):
                 L.colsum(buf.data_ptr() + 4 * sp.off('z'), sp.cstride, G['dzvec'], S * NB, buf.shape[2] * buf.shape[3], Zc, out_stride=Zp)
         if not hp.nz:
             return
-        nz, A = hp.nz, self.A
+        # the action and state slots' gradients are discarded: the states enter under stop_gradient (savp_model.py:414-421)
+        nz, off = hp.nz, self.A + self.Sd
         b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
         G['dzh'].zero_()
         for t in range(S - 1, -1, -1):
             # dh[t+1] = z-slot gradient (rnn_z part) + recurrent part already accumulated in dzh[t+1]
-            L.axpy_channels(G['dzvec'][t].data_ptr() + 4 * A, Zp, G['dzh'][t + 1].data_ptr(), nz, NB, nz)
+            L.axpy_channels(G['dzvec'][t].data_ptr() + 4 * off, Zp, G['dzh'][t + 1].data_ptr(), nz, NB, nz)
             L.lstm_cell_bwd(Bf['zgates'][t], Bf['zc'][t], Bf['zc'][t + 1], G['dzh'][t + 1], G['dzc'][t + 1] if t + 1 < S else None,
                             G['dzgates'][t], G['dzc'][t], NB, nz)
             L.dense_bwd(Bf['zcat'][t], 2 * nz, P[b + '/kernel'], G['dzgates'][t], 4 * nz, NB, 2 * nz, 4 * nz, dx=G['dzcat'][t],

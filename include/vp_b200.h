@@ -48,7 +48,9 @@ typedef struct vp_conv_geom {
 enum { VP_ACT_NONE = 0, VP_ACT_RELU = 1, VP_ACT_LRELU = 2, VP_ACT_SIGMOID = 3, VP_ACT_TANH = 4 };
 enum { VP_WKIND_PLAIN = 0, VP_WKIND_POOLED = 1, VP_WKIND_UPSAMPLED = 2 };
 enum { VP_WLAYOUT_FWD = 0, VP_WLAYOUT_DGRAD = 1,
-       VP_WLAYOUT_RESIDUAL = 4 /* OR-ed in: pack tf32(w - tf32(w)), the low part of the fp32-exact 3xTF32 mode */ };
+       VP_WLAYOUT_RESIDUAL = 4 /* OR-ed in: pack tf32(w - tf32(w)), the low part of the fp32-exact 3xTF32 mode */,
+       VP_WLAYOUT_GATES = 8    /* OR-ed in (FWD only, co = 4F, F % 32 == 0): GEMM column 128 t + 32 g + c holds gate g
+                                  (i, j, f, o) of cell channel 32 t + c -- the pack vp_conv_lstm_fwd reads */ };
 
 const char* vp_last_error(void);
 int vp_version(void);
@@ -74,6 +76,18 @@ int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const float* wpack
 int vp_conv_igemm_actgrad(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
                           const vp_tensor* out, const float* act_output, const float* addend, int act, float alpha,
                           int accumulate /* 0, or 2: the existing `out` is added to conv(in) first */, vp_stream_t stream);
+
+/* Norm-free ConvLSTM cell step (BasicConv2DLSTMCell with normalizer_fn=None, rnn_ops.py:115-126, 137-171): one
+ * launch of the engine above whose epilogue runs the whole cell from the accumulators.  wpacked is a VP_WLAYOUT_GATES
+ * pack (n_pad == 4F, F % 32 == 0); z is the dense [pixels][4F] gate pre-activation in natural order [i|j|f|o], with the
+ * pixels of the convolution's output; c_prev / c_new dense [pixels][F]; bias [4F] natural order:
+ *   z = conv(in) + bias,  c_new = c_prev sigmoid(f + forget_bias) + sigmoid(i) tanh(j),  h = tanh(c_new) sigmoid(o),
+ * h written to num_h_dst (1..3) channel slices h_dst[i] (16-byte aligned, channel stride h_cstride[i]).
+ * accumulate = 1: a partial pass of the fp32-exact mode, z += conv(in) only; accumulate = 2: z = z + conv(in) + bias, then
+ * the cell (the last pass).  Unsplit: identical inputs give identical bits. */
+int vp_conv_lstm_fwd(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc, const vp_tensor* z,
+                     const float* bias, const float* c_prev, float* c_new, float* const* h_dst, const int* h_cstride,
+                     int num_h_dst, float forget_bias, int accumulate, vp_stream_t stream);
 
 /* lo = x - tf32_truncate(x) over n floats (16-byte aligned, n % 4 == 0): the part of an fp32 activation the tensor core
  * does not read.  conv(x, W) + conv(lo, W) + conv(x, W_residual) is the fp32-exact ("3xTF32") debug mode. */
@@ -189,6 +203,13 @@ int vp_lstm_gates_bwd(const float* pre, int n, int positions, int filters, const
                       const float* stats2, float forget_bias, const float* const* dh, const int* dh_cstride,
                       int num_dh, const float* dc_next, float* dpre, float* dc_prev, float* dgamma1, float* dbeta1,
                       float* dgamma2, float* dbeta2, vp_stream_t stream);
+/* Backward of the norm-free ConvLSTM cell (vp_conv_lstm_fwd): z [rows][4F] natural order, c_prev / c_new / dc_next
+ * (may be NULL = 0) / dc_prev [rows][F] dense; dh = the sum of the num_dh (1..4) sources, added in list order.
+ * dz [rows][4F] and dc_prev are overwritten; no atomics (identical inputs give identical bits).  The bias gradient is
+ * vp_colsum of dz. */
+int vp_lstm_plain_bwd(const float* z, const float* c_prev, const float* c_new, long long rows, int filters,
+                      const float* const* dh, const int* dh_cstride, int num_dh, const float* dc_next, float* dz,
+                      float* dc_prev, float forget_bias, vp_stream_t stream);
 int vp_composite_bwd(const float* dgen, const float* masks, int masks_cstride, const float* layers, int layers_cstride,
                      float* dlogits, int dlogits_cstride, float* dlayers, int dlayers_cstride, long long positions,
                      int num_layers, vp_stream_t stream);

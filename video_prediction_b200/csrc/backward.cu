@@ -599,6 +599,32 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ gates, const floa
   dc_prev[idx] = dc * sf;
 }
 
+// norm-free ConvLSTM cell backward (vp_conv_lstm_fwd): one thread per (row, cell channel), dh summed in source order
+__global__ void lstm_plain_bwd_kernel(const float* __restrict__ z, const float* __restrict__ c_prev,
+                                      const float* __restrict__ c_new, SrcList dh, const float* __restrict__ dc_next,
+                                      float* __restrict__ dz, float* __restrict__ dc_prev, long long total, int F,
+                                      float forget_bias) {
+  for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long p = idx / F;
+    const int u = static_cast<int>(idx - p * F);
+    const float* g = z + p * 4 * F;
+    float* dg = dz + p * 4 * F;
+    const float si = sigm(g[u]), tj = tanhf(g[F + u]), sf = sigm(g[2 * F + u] + forget_bias), so = sigm(g[3 * F + u]);
+    const float th = tanhf(c_new[idx]);
+    float dhv = 0.f;
+#pragma unroll
+    for (int s = 0; s < 4; ++s)
+      if (s < dh.count) dhv += dh.ptr[s][p * dh.stride[s] + u];
+    const float dc = dhv * so * (1.f - th * th) + (dc_next ? dc_next[idx] : 0.f);
+    dg[u] = dc * tj * si * (1.f - si);
+    dg[F + u] = dc * si * (1.f - tj * tj);
+    dg[2 * F + u] = dc * c_prev[idx] * sf * (1.f - sf);
+    dg[3 * F + u] = dhv * th * so * (1.f - so);
+    dc_prev[idx] = dc * sf;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // reductions / elementwise
 // ------------------------------------------------------------------------------------------------
@@ -984,6 +1010,20 @@ extern "C" int vp_dense_bwd(const float* x, int x_stride, const float* w, const 
     }
   }
   return 0;
+}
+
+extern "C" int vp_lstm_plain_bwd(const float* z, const float* c_prev, const float* c_new, long long rows, int filters,
+                                 const float* const* dh, const int* dh_cstride, int num_dh, const float* dc_next, float* dz,
+                                 float* dc_prev, float forget_bias, vp_stream_t stream) {
+  if (!z || !c_prev || !c_new || !dh || !dh_cstride || !dz || !dc_prev) return set_error("vp_lstm_plain_bwd: null pointer");
+  if (rows < 1 || filters < 1 || num_dh < 1 || num_dh > 4) return set_error("vp_lstm_plain_bwd: bad rows / filters / source count");
+  for (int i = 0; i < num_dh; ++i)
+    if (!dh[i] || dh_cstride[i] < filters) return set_error("vp_lstm_plain_bwd: dh source %d is null or narrower than F", i);
+  const long long total = rows * filters;
+  const int blocks = static_cast<int>(std::min<long long>(16LL * device_sms(), (total + 255) / 256));
+  lstm_plain_bwd_kernel<<<blocks, 256, 0, as_stream(stream)>>>(z, c_prev, c_new, make_srcs(dh, dh_cstride, num_dh), dc_next,
+                                                              dz, dc_prev, total, filters, forget_bias);
+  return check_launch("lstm_plain_bwd_kernel");
 }
 
 extern "C" int vp_lstm_cell_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh, const float* dc_next,

@@ -61,6 +61,14 @@ struct alignas(64) IgemmArgs {
   int32_t aux_act;
   int32_t stages;
   int32_t k_tail;        // MMAs (K = 8 channels each) that hold real channels in the LAST k-chunk of a tap (1..4)
+  // ConvLSTM epilogue (vp_conv_lstm_fwd): `out` is the natural-order gate pre-activation z [pixels][4F]; GEMM column
+  // 128 t + 32 g + c of the GATES pack is gate g of cell channel 32 t + c
+  int32_t lstm_f, num_h;
+  float forget_bias;
+  const float* c_prev;
+  float* c_new;
+  float* h_dst[3];
+  int32_t h_cs[3];
   Tap taps[kMaxTaps];
 };
 
@@ -93,6 +101,45 @@ __device__ __forceinline__ void fwd_store(const IgemmArgs& a, long long ooff, in
   *o = a.accumulate == 1 ? *o + v : v;
 }
 
+__device__ __forceinline__ float sigm_fast(float v) { return 1.f / (1.f + __expf(-v)); }
+__device__ __forceinline__ float2 ld2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+__device__ __forceinline__ void st2(float* p, float x, float y) { *reinterpret_cast<float2*>(p) = make_float2(x, y); }
+
+// ConvLSTM epilogue of one pixel row (rnn_ops.py:137-171 without normalizer_fn).  With the GATES pack and BN = 128 the
+// thread's accumulators acc[4 (4 g + k) + 2 r + e] are gate g of cell channel 32 blockIdx.y + 8 k + 2 (lane % 4) + e, so
+// the whole cell runs from registers:  z = conv + bias (natural order [i|j|f|o], kept for the backward),
+// c' = c sigmoid(f + forget_bias) + sigmoid(i) tanh(j),  h = tanh(c') sigmoid(o).
+// accumulate = 1 is a partial pass of the fp32-exact mode (z += conv, nothing else); accumulate = 2 adds z first.
+__device__ __forceinline__ void lstm_store(const IgemmArgs& a, long long pix, const float* acc, int r, int lane) {
+  const int F = a.lstm_f;
+  float* z = a.out + pix * 4 * F;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int ch = 32 * blockIdx.y + 8 * k + 2 * (lane & 3);
+    float zx[4], zy[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) { zx[g] = acc[4 * (4 * g + k) + 2 * r]; zy[g] = acc[4 * (4 * g + k) + 2 * r + 1]; }
+    if (a.accumulate == 1) {
+#pragma unroll
+      for (int g = 0; g < 4; ++g) { const float2 o = ld2(z + g * F + ch); st2(z + g * F + ch, o.x + zx[g], o.y + zy[g]); }
+      continue;
+    }
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      if (a.accumulate == 2) { const float2 o = ld2(z + g * F + ch); zx[g] += o.x; zy[g] += o.y; }
+      const float2 b = __ldg(reinterpret_cast<const float2*>(a.bias + g * F + ch));
+      zx[g] += b.x; zy[g] += b.y;
+      st2(z + g * F + ch, zx[g], zy[g]);
+    }
+    const float2 cp = ld2(a.c_prev + pix * F + ch);
+    const float cx = cp.x * sigm_fast(zx[2] + a.forget_bias) + sigm_fast(zx[0]) * tanhf(zx[1]);
+    const float cy = cp.y * sigm_fast(zy[2] + a.forget_bias) + sigm_fast(zy[0]) * tanhf(zy[1]);
+    st2(a.c_new + pix * F + ch, cx, cy);
+    const float hx = tanhf(cx) * sigm_fast(zx[3]), hy = tanhf(cy) * sigm_fast(zy[3]);
+    for (int d = 0; d < a.num_h; ++d) st2(a.h_dst[d] + pix * a.h_cs[d] + ch, hx, hy);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // forward / dgrad kernel.  A CTA owns one (BN-column tile, phase, k-split) and walks the 128-pixel tiles
 // m = blockIdx.x, blockIdx.x + gridDim.x, ... (persistent): the TMA ring keeps streaming across tiles, so the loads of
@@ -100,7 +147,7 @@ __device__ __forceinline__ void fwd_store(const IgemmArgs& a, long long ooff, in
 // and a BN x 128 B weight tile, both 128B-swizzled.
 // ------------------------------------------------------------------------------------------------
 constexpr int kFwdThreads = 384;
-template <int BN>
+template <int BN, bool kLstm>
 __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_constant__ IgemmArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -217,6 +264,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
       const int od = (td * a.bd + ld[r]) * a.os_d + a.phase_ooff[phase][0];
       const int on = tn * a.bn + ln[r];
       if (ow < a.out_w && oh < a.out_h && od < a.out_d && on < a.out_n) {
+        if constexpr (kLstm) {
+          lstm_store(a, ((static_cast<long long>(on) * a.out_d + od) * a.out_h + oh) * a.out_w + ow, acc, r, lane);
+          continue;
+        }
         const long long ooff = on * a.so_n + od * a.so_d + oh * a.so_h + ow * a.so_w;
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
@@ -561,9 +612,20 @@ static int build_geometry(IgemmArgs& A, const vp_conv_geom* g, const vp_tensor* 
 
 using namespace vp;
 
+// The cell of vp_conv_lstm_fwd, for conv_igemm_impl (nullptr: a plain convolution).
+struct LstmCell {
+  const float* c_prev;
+  float* c_new;
+  float* const* h_dst;
+  const int* h_cs;
+  int num_h;
+  float forget_bias;
+};
+
 static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
                            const vp_tensor* out, const float* bias, int act, float alpha, int split_k, int accumulate,
-                           const float* aux_y, const float* aux_add, int aux_act, vp_stream_t stream) {
+                           const float* aux_y, const float* aux_add, int aux_act, vp_stream_t stream,
+                           const LstmCell* cell = nullptr) {
   if (check_tensor(in, "vp_conv_igemm(in)") || check_tensor(out, "vp_conv_igemm(out)")) return -1;
   if (!g || !wpacked) return set_error("vp_conv_igemm: null argument");
   if (n_pad % 16 || n_pad < 16) return set_error("vp_conv_igemm: n_pad must be a positive multiple of 16");
@@ -591,6 +653,12 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
       const int cols = ceil_div(n_pad, bn) * bn;
       if (cols < best) { best = cols; A.bn_tile = bn; }
     }
+  }
+  if (cell) {     // a 128-column tile holds all four gates of 32 cell channels
+    A.bn_tile = 128;
+    A.lstm_f = out->c / 4;
+    A.c_prev = cell->c_prev; A.c_new = cell->c_new; A.num_h = cell->num_h; A.forget_bias = cell->forget_bias;
+    for (int i = 0; i < cell->num_h; ++i) { A.h_dst[i] = cell->h_dst[i]; A.h_cs[i] = cell->h_cs[i]; }
   }
   const int n_tiles = ceil_div(n_pad, A.bn_tile);
   int min_iters = 1 << 30;
@@ -628,7 +696,8 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
   A.stages = static_cast<int>(std::min<size_t>(kMaxStagesFwd, (smem_max - 1024) / stage_bytes));
   const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
   typedef void (*FwdKernel)(const IgemmArgs);
-  static const FwdKernel kernels[3] = {igemm_fwd_kernel<32>, igemm_fwd_kernel<64>, igemm_fwd_kernel<128>};
+  static const FwdKernel kernels[4] = {igemm_fwd_kernel<32, false>, igemm_fwd_kernel<64, false>, igemm_fwd_kernel<128, false>,
+                                       igemm_fwd_kernel<128, true>};
   static bool attr_set = false;
   if (!attr_set) {
     for (FwdKernel k : kernels)
@@ -636,7 +705,7 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
         return set_error("cudaFuncSetAttribute(igemm_fwd_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
     attr_set = true;
   }
-  const FwdKernel kernel = kernels[A.bn_tile == 32 ? 0 : A.bn_tile == 64 ? 1 : 2];
+  const FwdKernel kernel = kernels[cell ? 3 : A.bn_tile == 32 ? 0 : A.bn_tile == 64 ? 1 : 2];
   // persistent over the pixel tiles: one CTA per SM in total; each CTA strides through the M tiles
   const int m_tiles = A.tiles_w * A.tiles_h * A.tiles_d * A.tiles_n;
   const int other = n_tiles * A.num_phases * A.splits;
@@ -659,6 +728,24 @@ extern "C" int vp_conv_igemm_actgrad(const vp_tensor* in, const vp_conv_geom* g,
   if (out->c != out->cstride) return set_error("vp_conv_igemm_actgrad: dense output required");
   if (accumulate != 0 && accumulate != 2) return set_error("vp_conv_igemm_actgrad: accumulate must be 0 or 2");
   return conv_igemm_impl(in, g, wpacked, n_pad, kc, out, nullptr, VP_ACT_NONE, alpha, 1, accumulate, act_output, addend, act, stream);
+}
+
+extern "C" int vp_conv_lstm_fwd(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
+                                const vp_tensor* z, const float* bias, const float* c_prev, float* c_new, float* const* h_dst,
+                                const int* h_cstride, int num_h_dst, float forget_bias, int accumulate, vp_stream_t stream) {
+  if (check_tensor(z, "vp_conv_lstm_fwd(z)")) return -1;
+  if (z->c % 128) return set_error("vp_conv_lstm_fwd: the cell needs filters %% 32 == 0 (got %d)", z->c / 4);
+  if (z->c != z->cstride || n_pad != z->c) return set_error("vp_conv_lstm_fwd: z must be dense [pixels][4F] and n_pad == 4F");
+  if (!bias || !c_prev || !c_new || !h_dst || !h_cstride) return set_error("vp_conv_lstm_fwd: null argument");
+  if (num_h_dst < 1 || num_h_dst > 3) return set_error("vp_conv_lstm_fwd: 1 to 3 h destinations (got %d)", num_h_dst);
+  if ((reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(c_prev) | reinterpret_cast<uintptr_t>(c_new)) & 15)
+    return set_error("vp_conv_lstm_fwd: bias / c pointers must be 16B aligned");
+  for (int i = 0; i < num_h_dst; ++i)
+    if (!h_dst[i] || (reinterpret_cast<uintptr_t>(h_dst[i]) & 15) || h_cstride[i] < z->c / 4 || (h_cstride[i] & 3))
+      return set_error("vp_conv_lstm_fwd: h destination %d: null, unaligned, or channel stride below F / not a multiple of 4", i);
+  if (accumulate < 0 || accumulate > 2) return set_error("vp_conv_lstm_fwd: accumulate must be 0, 1 or 2 (got %d)", accumulate);
+  const LstmCell cell{c_prev, c_new, h_dst, h_cstride, num_h_dst, forget_bias};
+  return conv_igemm_impl(in, g, wpacked, n_pad, kc, z, bias, VP_ACT_NONE, 0.f, 1, accumulate, nullptr, nullptr, 0, stream, &cell);
 }
 
 extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked,

@@ -7,6 +7,8 @@
 //   UPSAMPLED  upsample_conv2d (ops.py:698-704): bilinear 4x4 (x) kernel, FULL correlation
 // and stored K-major, zero padded and rounded to TF32 (round-to-nearest), in the layout the wgmma
 // descriptors read:  FWD  [tap][co -> n_pad][ci -> kc*32],  DGRAD [tap][ci -> n_pad][co -> kc*32].
+// A ConvLSTM's forward packs may interleave the four gates (VP_WLAYOUT_GATES) so that the engine's epilogue holds every
+// gate of a cell channel in one thread.
 // A channel map lets the engine's internal (16-byte aligned, padded) concat layouts differ from the
 // reference's channel order.
 #include <algorithm>
@@ -57,8 +59,10 @@ __device__ __forceinline__ void pack_element(const float* __restrict__ w, int kd
   const int k = static_cast<int>(idx % kpad);
   const int n = static_cast<int>((idx / kpad) % n_pad);
   const int tap = static_cast<int>(idx / (static_cast<long long>(kpad) * n_pad));
-  const int co = (layout & 3) == VP_WLAYOUT_FWD ? n : k;
+  int co = (layout & 3) == VP_WLAYOUT_FWD ? n : k;
   const int ci = (layout & 3) == VP_WLAYOUT_FWD ? k : n;
+  // VP_WLAYOUT_GATES: GEMM column 128 t + 32 g + c holds gate g of cell channel 32 t + c (co = 4F, natural order [i|j|f|o])
+  if ((layout & VP_WLAYOUT_GATES) && co < co_n) co = ((co & 127) >> 5) * (co_n >> 2) + 32 * (co >> 7) + (co & 31);
   float v = 0.f;
   if (co < co_n && ci < ci_int) {
     const int cr = cmap ? cmap[ci] : ci;
@@ -166,6 +170,8 @@ extern "C" int vp_pack_weights(const float* w, int kd, int kh, int kw, int ci_re
   const int kpad = kc * 32;
   const int rows = (layout & 3) == VP_WLAYOUT_FWD ? co : ci_int, cols = (layout & 3) == VP_WLAYOUT_FWD ? ci_int : co;
   if (rows > n_pad || cols > kpad) return set_error("vp_pack_weights: n_pad/kc too small (%d>%d or %d>%d)", rows, n_pad, cols, kpad);
+  if ((layout & VP_WLAYOUT_GATES) && ((layout & 3) != VP_WLAYOUT_FWD || co % 128))
+    return set_error("vp_pack_weights: the GATES layout is a forward layout of 4F columns with F %% 32 == 0 (co = %d)", co);
   const long long total = static_cast<long long>(taps) * n_pad * kpad;
   pack_weights_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(w, kd, kh, kw, ci_ref, co, kind, layout, cmap,
                                                                          ci_int, inv_scale, wpacked, taps, n_pad, kpad);

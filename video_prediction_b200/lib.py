@@ -30,6 +30,7 @@ ACT_NONE, ACT_RELU, ACT_LRELU, ACT_SIGMOID, ACT_TANH = range(5)
 WKIND_PLAIN, WKIND_POOLED, WKIND_UPSAMPLED = range(3)
 WLAYOUT_FWD, WLAYOUT_DGRAD = range(2)
 WLAYOUT_RESIDUAL = 4
+WLAYOUT_GATES = 8        # OR-ed into a forward layout: the gate-interleaved pack of a ConvLSTM (vp_conv_lstm_fwd)
 
 
 class VpError(RuntimeError):
@@ -156,6 +157,21 @@ def conv_igemm_actgrad(x_view, g, wpacked, n_pad, kc, out_view, act_output_addr,
               lambda: check(lib().vp_conv_igemm_actgrad(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(out_view),
                                                         C.c_void_p(act_output_addr), C.c_void_p(addend_addr or 0), act,
                                                         C.c_float(alpha), int(accumulate), stream_ptr())))
+
+
+def conv_lstm_fwd(x_view, g, wpacked, n_pad, kc, z, bias, c_prev, c_new, h_dsts, accumulate=0, forget_bias=1.0):
+    """Norm-free ConvLSTM step (vp_conv_lstm_fwd): z [.., 4F] (dense, natural gate order) = conv + bias, c_new and h
+    from the engine's epilogue.  h_dsts: list of (address:int, cstride:int).  wpacked is a WLAYOUT_GATES pack."""
+    if 'igemm' in _SKIP:
+        return
+    zv = tensor_view(z.view((-1,) + tuple(z.shape[-3:])))
+    k = len(h_dsts)
+    pa = (C.c_void_p * k)(*[C.c_void_p(a) for a, _ in h_dsts])
+    sa = (C.c_int * k)(*[s for _, s in h_dsts])
+    _profiled('igemm', _conv_flops(x_view, g, zv),
+              lambda: check(lib().vp_conv_lstm_fwd(C.byref(x_view), C.byref(g), ptr(wpacked), n_pad, kc, C.byref(zv), ptr(bias),
+                                                   ptr(c_prev), ptr(c_new), pa, sa, k, _f(forget_bias), int(accumulate),
+                                                   stream_ptr())))
 
 
 def tf32_residual(x):
@@ -401,6 +417,15 @@ def lstm_gates_bwd(pre, n, positions, filters, c_prev, g1, b1, g2, b2, stats1, s
     check(lib().vp_lstm_gates_bwd(ptr(pre), n, positions, filters, ptr(c_prev), ptr(g1), ptr(b1), ptr(g2), ptr(b2), ptr(stats1),
                                   ptr(stats2), _f(forget_bias), pa, sa, k, ptr(dc_next), ptr(dpre), ptr(dc_prev), ptr(dg1),
                                   ptr(db1), ptr(dg2), ptr(db2), stream_ptr()))
+
+
+def lstm_plain_bwd(z, c_prev, c_new, rows, filters, dh_srcs, dc_next, dz, dc_prev, forget_bias=1.0):
+    """Backward of vp_conv_lstm_fwd's cell: dz (natural order) and dc_prev overwritten; dh = sum of dh_srcs in order."""
+    if 'gates' in _SKIP:
+        return
+    pa, sa, k = _srcs(dh_srcs)
+    check(lib().vp_lstm_plain_bwd(ptr(z), ptr(c_prev), ptr(c_new), C.c_longlong(rows), filters, pa, sa, k, ptr(dc_next), ptr(dz),
+                                  ptr(dc_prev), _f(forget_bias), stream_ptr()))
 
 
 def composite_bwd(dgen, masks, masks_cs, layers_addr, layers_cs, dlogits, dlogits_cs, dlayers, dlayers_cs, positions, num_layers):

@@ -70,7 +70,7 @@ class ConvLayer(object):
     (cmap None = identity).  `inv_scale` (optional device scalar, the spectral-norm sigma) divides the weights in every pack.
     In the fp32-exact mode (`model.exact`) every call runs as three TF32 passes (conv3x) against the residual packs."""
 
-    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co, inv_scale=None):
+    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co, inv_scale=None, gates=False):
         self.model, self.wname, self.bname = model, wname, bname
         self.k, self.kind, self.stride, self.pad, self.transposed = k, kind, stride, pad, transposed
         self.co, self.inv_scale = co, inv_scale
@@ -85,8 +85,10 @@ class ConvLayer(object):
         self.nd = 3 if (self.ke[0], stride[0], pad[0]) == (1, 1, 0) else 4
         self.geom = L.geom(self.ke, stride, pad, transposed)
         self.cmap = None if cmap is None else torch.tensor(cmap, dtype=torch.int32, device=model.device)
-        self.wp, self.n_pad, self.kc = self._alloc(L.WLAYOUT_FWD)
-        self.wp_lo = self._alloc(L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL)[0] if model.exact else None
+        # gates: the forward packs of a norm-free ConvLSTM interleave its four gates for the cell epilogue (lstm_fwd)
+        self.fwd_layout = L.WLAYOUT_FWD | (L.WLAYOUT_GATES if gates else 0)
+        self.wp, self.n_pad, self.kc = self._alloc(self.fwd_layout)
+        self.wp_lo = self._alloc(self.fwd_layout | L.WLAYOUT_RESIDUAL)[0] if model.exact else None
         self.wpd = self.wpd_lo = None
 
     def _alloc(self, layout):
@@ -105,7 +107,7 @@ class ConvLayer(object):
     def pack_jobs(self):
         """PackPlan entries that fill every packed buffer of this layer from its reference-layout weights."""
         w = self.model.params[self.wname]
-        bufs = ((L.WLAYOUT_FWD, self.wp), (L.WLAYOUT_FWD | L.WLAYOUT_RESIDUAL, self.wp_lo),
+        bufs = ((self.fwd_layout, self.wp), (self.fwd_layout | L.WLAYOUT_RESIDUAL, self.wp_lo),
                 (L.WLAYOUT_DGRAD, self.wpd), (L.WLAYOUT_DGRAD | L.WLAYOUT_RESIDUAL, self.wpd_lo))
         return [(w, self.k, self.ci_ref, self.co, self.kind, layout, self.ci_int, self.cmap, self.inv_scale, out)
                 for layout, out in bufs if out is not None]
@@ -120,6 +122,22 @@ class ConvLayer(object):
             conv3x(x, self.ci_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, ov, bias, act, alpha)
             return
         L.conv_igemm(xv, self.geom, self.wp, self.n_pad, self.kc, ov, bias, act, alpha, split_k)
+
+    def lstm_fwd(self, x, z, c_prev, c_new, h_dests):
+        """One norm-free ConvLSTM step from the GATES packs: z = conv(x) + bias (natural gate order), c_new and h (to the
+        (address, cstride) slices h_dests) from the engine's epilogue.  fp32-exact mode: two partial passes add into a
+        zeroed z, the third adds the residual-weight pass and runs the cell."""
+        x = self._view(x)
+        xv = L.tensor_view(x, self.ci_int)
+        cell = (z, self.model.params[self.bname], c_prev, c_new, h_dests)
+        if self.model.exact:
+            z.zero_()
+            L.conv_lstm_fwd(xv, self.geom, self.wp, self.n_pad, self.kc, *cell, accumulate=1)
+            L.conv_lstm_fwd(L.tensor_view(L.tf32_residual(x), self.ci_int), self.geom, self.wp, self.n_pad, self.kc, *cell,
+                            accumulate=1)
+            L.conv_lstm_fwd(xv, self.geom, self.wp_lo, self.n_pad, self.kc, *cell, accumulate=2)
+            return
+        L.conv_lstm_fwd(xv, self.geom, self.wp, self.n_pad, self.kc, *cell)
 
     def dgrad(self, dy, dx, dy_c=None, accumulate=False, act_y=None, addend=None, act=L.ACT_NONE, alpha=0.0):
         """dx[.., ci_int] (+)= conv^T(dy): the same engine with the transposed flag flipped.  With act_y, the output of the
@@ -218,19 +236,26 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise ValueError('Unknown GAN loss type %s' % hp.gan_loss_type)                 # losses.py:52-53
         unsupported = []
         for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('conv_rnn_norm_layer', 'instance'),
+                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'),
                           ('norm_layer', 'instance'), ('downsample_layer', 'conv_pool2d'),
                           ('upsample_layer', 'upsample_conv2d'), ('activation_layer', 'relu'), ('last_frames', 1),
                           ('prev_image_background', True), ('first_image_background', True),
                           ('last_image_background', False), ('last_context_image_background', False),
                           ('context_images_background', False), ('generate_scratch_image', True),
                           ('dependent_mask', True), ('use_e_rnn', False), ('learn_prior', False),
-                          ('learn_initial_state', False), ('ablation_conv_rnn_norm', False), ('ablation_rnn', False),
+                          ('learn_initial_state', False), ('ablation_rnn', False),
                           ('use_rnn_z', True), ('joint_gan_optimization', False), ('use_same_discriminator', False)):
             # (`repeat` is accepted with any value: train.py sets it to the dataset's time_shift (train.py:160) and no model
             #  code of the reference reads it, base_model.py:90-95)
             if getattr(hp, key) != want:
                 unsupported.append('%s=%r' % (key, getattr(hp, key)))
+        # the ConvLSTM's normalisation (savp_model.py:370-390): instance norms inside the cell, none, or (ablation) one
+        # instance norm on the cell's output
+        if hp.conv_rnn_norm_layer not in ('instance', 'none'):
+            unsupported.append('conv_rnn_norm_layer=%r' % (hp.conv_rnn_norm_layer,))
+        elif hp.ablation_conv_rnn_norm and hp.conv_rnn_norm_layer == 'none':
+            raise ValueError('ablation_conv_rnn_norm=True needs a conv_rnn_norm_layer to apply to the cell output, got '
+                             "'none'")   # the reference calls None(h) (savp_model.py:380-383)
         if hp.transformation not in ('cdna', 'flow'):
             unsupported.append('transformation=%r' % (hp.transformation,))
         if tuple(hp.dilation_rate) != (1, 1):
@@ -246,6 +271,12 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 unsupported.append('kl_anneal=%r' % (hp.kl_anneal,))
         if unsupported:
             raise NotImplementedError('hparams outside the H100 hot path (SURVEY.md 8f): ' + ', '.join(unsupported))
+
+    @property
+    def cell_norm(self):
+        """True: the reference's default ConvLSTM, with instance norms inside the cell.  False: the norm-free cell
+        (conv_rnn_norm_layer='none', or the ablation_conv_rnn_norm form), whose gate math runs in the engine's epilogue."""
+        return self.hparams.conv_rnn_norm_layer == 'instance' and not self.hparams.ablation_conv_rnn_norm
 
     # ------------------------------------------------------------------ structure (savp_model.py:182-232)
     @staticmethod
@@ -301,8 +332,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         def lstm(i, cin, oc):
             b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, i)
             specs[b + '/kernel'] = ((5, 5, cin + Zc + oc, 4 * oc), 'kernel')
-            norm(b + '/input_transform_forget_output', 4 * oc)
-            norm(b + '/state', oc)
+            if self.cell_norm:
+                norm(b + '/input_transform_forget_output', 4 * oc)
+                norm(b + '/state', oc)
+            else:       # norm-free cell: the gate convolution has a bias (rnn_ops.py:122-125)
+                specs[b + '/bias'] = ((4 * oc,), 'zeros')
+                if hp.ablation_conv_rnn_norm:      # instance norm of the cell output h (savp_model.py:380-383)
+                    norm('%s/lstm_h%d/InstanceNorm' % (sc, i), oc)
         outs = []
         cin = 2 * C
         for i, (oc, use) in enumerate(enc):
@@ -689,14 +725,20 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 d['rin_spec'] = ConcatSpec([('x', oc)] + zseg + [('h', oc)])
                 Bf['rin%d' % li] = self._z(S + 1, NB, hh, ww, d['rin_spec'].cstride)
                 b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, li)
-                d['rconv'] = ConvLayer(self, b + '/kernel', None, (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1), (0, 2, 2), False,
-                                       d['rin_spec'], 4 * oc)
+                plain = not self.cell_norm
+                d['rconv'] = ConvLayer(self, b + '/kernel', b + '/bias' if plain else None, (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
+                                       (0, 2, 2), False, d['rin_spec'], 4 * oc, gates=plain)
                 d['rname'] = b
                 self.convs.append(d['rconv'])
                 Bf['gpre%d' % li] = self._z(S, NB, hh, ww, 4 * oc)
                 Bf['c%d' % li] = self._z(S + 1, NB, hh, ww, oc)      # c[t] = state entering step t
-                Bf['gst1_%d' % li] = self._z(S, NB, 4 * oc, 2)
-                Bf['gst2_%d' % li] = self._z(S, NB, oc, 2)
+                if self.cell_norm:
+                    Bf['gst1_%d' % li] = self._z(S, NB, 4 * oc, 2)
+                    Bf['gst2_%d' % li] = self._z(S, NB, oc, 2)
+                elif hp.ablation_conv_rnn_norm:
+                    # IN(h): the layer's output, copied to its consumers; the raw h is the recurrent state only
+                    Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
+                    Bf['hst%d' % li] = self._z(S, NB, oc, 2)
             else:
                 Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
             outs.append(oc)
@@ -1094,12 +1136,24 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 L.inorm_act(pre.data_ptr(), oc, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc,
                             P[nm + '/gamma'], P[nm + '/beta'], L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
                 gpre = Bf['gpre%d' % li][t]
-                d['rconv'].fwd(rin, gpre)
                 b = d['rname']
-                L.lstm_gates_fwd(gpre, NB, hh * ww, oc, Bf['c%d' % li][t],
-                                 P[b + '/input_transform_forget_output/gamma'], P[b + '/input_transform_forget_output/beta'],
-                                 P[b + '/state/gamma'], P[b + '/state/beta'], Bf['c%d' % li][t + 1], self._h_dests(li, t),
-                                 Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t])
+                if self.cell_norm:
+                    d['rconv'].fwd(rin, gpre)
+                    L.lstm_gates_fwd(gpre, NB, hh * ww, oc, Bf['c%d' % li][t],
+                                     P[b + '/input_transform_forget_output/gamma'], P[b + '/input_transform_forget_output/beta'],
+                                     P[b + '/state/gamma'], P[b + '/state/beta'], Bf['c%d' % li][t + 1], self._h_dests(li, t),
+                                     Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t])
+                elif hp.ablation_conv_rnn_norm:
+                    dests = self._h_dests(li, t)
+                    d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], dests[:1])
+                    nm = '%s/lstm_h%d/InstanceNorm' % (sc, li)
+                    out = Bf['out%d' % li][t]
+                    L.inorm_act(dests[0][0], dests[0][1], out.data_ptr(), oc, NB, hh * ww, oc, P[nm + '/gamma'], P[nm + '/beta'],
+                                L.ACT_NONE, 0.0, Bf['hst%d' % li][t])
+                    for a, cs in dests[1:]:
+                        L.copy_channels(out.data_ptr(), oc, a, cs, NB * hh * ww, oc)
+                else:
+                    d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], self._h_dests(li, t))
             else:
                 dests = self._h_dests(li, t)
                 out = Bf['out%d' % li][t]

@@ -216,6 +216,8 @@ class TrainMixin(object):
                 G['drin%d' % li] = torch.zeros_like(Bf['rin%d' % li])
                 G['dgpre%d' % li] = torch.zeros_like(Bf['gpre%d' % li])
                 G['dc%d' % li] = torch.zeros_like(Bf['c%d' % li])
+                if 'hst%d' % li in Bf:       # ablation_conv_rnn_norm: gradient of the raw h from the downstream consumers
+                    G['dhn%d' % li] = torch.zeros_like(Bf['out%d' % li])
         ngf = hp.ngf
         G['dgen'] = z(S, NB, H, W, 4)
         G['dimg'] = z(S, NB, H, W, 4)
@@ -388,7 +390,21 @@ class TrainMixin(object):
             if li == n_enc - 1 and not self.flow:
                 srcs.append((G['dsmall'][t].data_ptr(), oc))
             nm = '%s/h%d/InstanceNorm' % (sc, li)
-            if d['use']:
+            if d['use'] and not self.cell_norm:
+                rsp = d['rin_spec']
+                if 'hst%d' % li in Bf:    # h -> IN(h) -> consumers: their gradient through the norm, before the recurrent one
+                    nm_h = '%s/lstm_h%d/InstanceNorm' % (sc, li)
+                    L.inorm_act_bwd(Bf['rin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride, srcs,
+                                    G['dhn%d' % li][t].data_ptr(), oc, NB, hh * ww, oc, P[nm_h + '/gamma'], P[nm_h + '/beta'],
+                                    Bf['hst%d' % li][t], L.ACT_NONE, 0.0, Gp[nm_h + '/gamma'], Gp[nm_h + '/beta'])
+                    srcs = [(G['dhn%d' % li][t].data_ptr(), oc)]
+                if t + 1 < S:
+                    srcs.append((G['drin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride))
+                L.lstm_plain_bwd(Bf['gpre%d' % li][t], Bf['c%d' % li][t], Bf['c%d' % li][t + 1], NB * hh * ww, oc, srcs,
+                                 G['dc%d' % li][t + 1] if t + 1 < S else None, G['dgpre%d' % li][t], G['dc%d' % li][t])
+                d['rconv'].dgrad(G['dgpre%d' % li][t], G['drin%d' % li][t])
+                srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
+            elif d['use']:
                 rsp = d['rin_spec']
                 if t + 1 < S:
                     srcs.append((G['drin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride))
@@ -436,6 +452,9 @@ class TrainMixin(object):
             L.colsum(G['dpre%d' % li].data_ptr(), d['oc'], Gp[d['conv'].bname], 1, S * NB * d['h'] * d['w'], d['oc'])
             if d['use']:
                 d['rconv'].wgrad(Bf['rin%d' % li][:S], G['dgpre%d' % li])
+                if d['rconv'].bname:      # norm-free cell: the gate convolution's bias
+                    L.colsum(G['dgpre%d' % li].data_ptr(), 4 * d['oc'], Gp[d['rconv'].bname], 1, S * NB * d['h'] * d['w'],
+                             4 * d['oc'])
             if red is not None:
                 pre = ('%s/h%d/' % (sc_cell, li), '%s/lstm_h%d/' % (sc_cell, li))
                 lo, hi = self._flat_range(self.g_flat, [k for k in P if k.startswith(pre)])

@@ -141,6 +141,13 @@ int vp_unpack_wgrad(const float* dwpacked, int kd, int kh, int kw, int ci_ref, i
 int vp_inorm_act(const float* x, int x_cstride, float* y, int y_cstride, int n, int positions, int c,
                  const float* gamma, const float* beta, float eps, int act, float alpha, float* stats,
                  vp_stream_t stream);
+/* tf.contrib.layers.layer_norm (+ activation) with begin_norm_axis=1, begin_params_axis=-1 (norm_layer='layer'):
+ * the same arguments, but mean / biased variance over all positions AND channels of a sample, gamma / beta per channel
+ * (eps 1e-12 in the reference).  stats (optional): [n][2] = (mean, rstd).  c % 4 == 0, c <= 4096; n, positions >= 1.
+ * Fixed summation order (identical inputs give identical bits); no host synchronisation. */
+int vp_lnorm_act(const float* x, int x_cstride, float* y, int y_cstride, int n, int positions, int c,
+                 const float* gamma, const float* beta, float eps, int act, float alpha, float* stats,
+                 vp_stream_t stream);
 
 /* BasicConv2DLSTMCell gate math, rnn_ops.py:148-165 (instance norm over the 4F concat, i/j/f/o
  * split, forget bias, instance norm of new_c, h = tanh(c)*sigmoid(o)).  pre: conv output
@@ -196,6 +203,12 @@ int vp_composite(const float* logits, int logits_cstride, const float* layers, i
  * Gradient inputs that have several consumers are passed as lists of (pointer, channel stride)
  * "sources" which the kernel sums.  Parameter gradients (dgamma, dbeta, dw, db ...) are ACCUMULATED. */
 int vp_inorm_act_bwd(const float* x, int x_cstride, const float* const* dy, const int* dy_cstride, int num_dy,
+                     float* dx, int dx_cstride, int n, int positions, int c, const float* gamma, const float* beta,
+                     const float* stats, int act, float alpha, float* dgamma, float* dbeta, vp_stream_t stream);
+/* Backward of vp_lnorm_act (stats [n][2] from its forward): dy = the sum of the num_dy (1..4) sources in list order;
+ * dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) with g = gamma * dy * act', means over the sample; dx overwritten
+ * (may alias x or a source), dgamma / dbeta ACCUMULATED.  No float atomics. */
+int vp_lnorm_act_bwd(const float* x, int x_cstride, const float* const* dy, const int* dy_cstride, int num_dy,
                      float* dx, int dx_cstride, int n, int positions, int c, const float* gamma, const float* beta,
                      const float* stats, int act, float alpha, float* dgamma, float* dbeta, vp_stream_t stream);
 int vp_lstm_gates_bwd(const float* pre, int n, int positions, int filters, const float* c_prev, const float* gamma1,

@@ -792,4 +792,260 @@ int slab_gates_bwd(const float* pre, int n, int P, int F, const float* c_prev, c
   return rc;
 }
 
+// ------------------------------------------------------------------------------------------------ layer norm
+// tf.contrib.layers.layer_norm (begin_norm_axis=1, begin_params_axis=-1): mean and biased variance over every position AND
+// channel of a sample, gamma / beta per channel.  A cluster of cs CTAs owns one sample, CTA `rank` walks the positions
+// [rank * ppc, min(P, (rank + 1) * ppc)); thread = (lane, quad of 4 channels), lanes * C/4 threads rounded up to whole
+// warps, so a thread's gamma / beta and its per-channel backward sums stay in registers.  The two per-sample scalars are
+// reduced through DSMEM with every CTA adding the partials in rank order, so all CTAs hold bit-identical totals.  A sample
+// is too large for registers at 64x64 and 128x128 (131072 - 524288 floats), so every shape takes two passes over x, the
+// second one served by the L2.  The cluster size depends on the shape only: the summation order is a function of the call.
+constexpr int kLnMaxThreads = 1024;
+
+struct LnPlan { int cs, ppc, lanes, threads; };
+
+static bool plan_lnorm(int P, int C, LnPlan* pl) {
+  const int c4 = C / 4;
+  if (c4 > kLnMaxThreads) return false;
+  pl->lanes = c4 >= 256 ? 1 : 256 / c4;
+  pl->threads = (pl->lanes * c4 + 31) / 32 * 32;
+  const long long e = static_cast<long long>(P) * C;
+  int cs = 1;
+  while (cs < 8 && static_cast<long long>(cs) * 4096 < e && cs * 2 <= P) cs *= 2;
+  pl->cs = cs;
+  pl->ppc = (P + cs - 1) / cs;
+  return true;
+}
+
+// (a, b) <- their sums over the cluster: warps in order, then the CTAs' partials in rank order.  s_warp [32][2], s_part [2].
+__device__ __forceinline__ void ln_reduce2(float& a, float& b, float* s_warp, float* s_part, float* s_tot, int cs) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+  if (lane == 0) { s_warp[2 * warp] = a; s_warp[2 * warp + 1] = b; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float ta = 0.f, tb = 0.f;
+    for (int w = 0; w < nw; ++w) { ta += s_warp[2 * w]; tb += s_warp[2 * w + 1]; }
+    s_part[0] = ta; s_part[1] = tb;
+  }
+  if (cs > 1) {
+    cg::cluster_group cluster = cg::this_cluster();
+    cluster.sync();
+    if (threadIdx.x == 0) {
+      float ta = 0.f, tb = 0.f;
+      for (int r = 0; r < cs; ++r) {
+        const float* peer = cluster.map_shared_rank(s_part, r);
+        ta += peer[0]; tb += peer[1];
+      }
+      s_tot[0] = ta; s_tot[1] = tb;
+    }
+  } else {
+    __syncthreads();
+    if (threadIdx.x == 0) { s_tot[0] = s_part[0]; s_tot[1] = s_part[1]; }
+  }
+  __syncthreads();
+  a = s_tot[0];
+  b = s_tot[1];
+}
+
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+
+// grid = n clusters of cs CTAs along x.  stats [n][2] = (mean, rstd).
+__global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_kernel(const float* __restrict__ x, int xs, float* __restrict__ y, int ys, int P,
+                                                                  int C, const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                                  float eps, int act, float alpha, float* __restrict__ stats, int lanes,
+                                                                  int ppc, int cs) {
+  __shared__ float s_warp[64], s_part[2], s_tot[2];
+  const int c4 = C >> 2, n = blockIdx.x / cs, rank = blockIdx.x % cs;
+  const bool active = threadIdx.x < lanes * c4;
+  const int q = threadIdx.x % c4, l = threadIdx.x / c4;
+  const int p0 = rank * ppc, p1 = min(P, p0 + ppc);
+  const float* xp = x + static_cast<long long>(n) * P * xs + 4 * q;
+  const float k = x[static_cast<long long>(n) * P * xs];             // shift: the sample's first value
+  float a = 0.f, b = 0.f;
+  if (active) {
+#pragma unroll 4
+    for (int p = p0 + l; p < p1; p += lanes) {
+      const float4 v = ld4(xp + static_cast<long long>(p) * xs);
+      const float d0 = v.x - k, d1 = v.y - k, d2 = v.z - k, d3 = v.w - k;
+      a += (d0 + d1) + (d2 + d3);
+      b += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+    }
+  }
+  ln_reduce2(a, b, s_warp, s_part, s_tot, cs);
+  const float inv = 1.f / (static_cast<float>(P) * C);
+  const float md = a * inv;                                          // mean - k
+  const float var = fmaxf(b * inv - md * md, 0.f);
+  const float m = k + md, r = rsqrtf(var + eps);
+  if (stats && rank == 0 && threadIdx.x == 0) { stats[2LL * n] = m; stats[2LL * n + 1] = r; }
+  if (active) {
+    float g[4], bb[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      g[i] = (gamma ? gamma[4 * q + i] : 1.f) * r;
+      bb[i] = (beta ? beta[4 * q + i] : 0.f) - m * g[i];
+    }
+    float* yp = y + static_cast<long long>(n) * P * ys + 4 * q;
+#pragma unroll 4
+    for (int p = p0 + l; p < p1; p += lanes) {
+      const float4 v = ld4(xp + static_cast<long long>(p) * xs);
+      float4 o;
+      o.x = p_act(v.x * g[0] + bb[0], act, alpha); o.y = p_act(v.y * g[1] + bb[1], act, alpha);
+      o.z = p_act(v.z * g[2] + bb[2], act, alpha); o.w = p_act(v.w * g[3] + bb[3], act, alpha);
+      *reinterpret_cast<float4*>(yp + static_cast<long long>(p) * ys) = o;
+    }
+  }
+  if (cs > 1) cg::this_cluster().sync();      // keep this CTA's shared memory alive until every peer has read its partials
+}
+
+// dyp = dy * act'(gamma * xh + beta), gy = gamma * dyp:  dx = r * (gy - mean(gy) - xh * mean(gy * xh)) over the sample.
+// The per-channel sums of dyp * xh and dyp: lanes in order within a CTA, then rank 0 adds the CTAs' rows in rank order
+// through DSMEM into row n of wg / wb.  dx may alias x or a dy source: every element is read and written by the same
+// thread, and read before it is written.
+__global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_bwd_kernel(const float* __restrict__ x, int xs, SlabSrcs srcs, float* dx, int dxs,
+                                                                      int P, int C, const float* __restrict__ gamma,
+                                                                      const float* __restrict__ beta, const float* __restrict__ stats,
+                                                                      int act, float alpha, float* __restrict__ wg, float* __restrict__ wb,
+                                                                      int lanes, int ppc, int cs) {
+  extern __shared__ float s_ch[];                                    // [threads][8] per-thread channel sums, then [2][C] the CTA's
+  __shared__ float s_warp[64], s_part[2], s_tot[2];
+  const int c4 = C >> 2, n = blockIdx.x / cs, rank = blockIdx.x % cs;
+  const bool active = threadIdx.x < lanes * c4;
+  const int q = threadIdx.x % c4, l = threadIdx.x / c4;
+  const int p0 = rank * ppc, p1 = min(P, p0 + ppc);
+  const float m = stats[2LL * n], r = stats[2LL * n + 1];
+  const float* xp = x + static_cast<long long>(n) * P * xs + 4 * q;
+  float g[4] = {0.f, 0.f, 0.f, 0.f}, be[4] = {0.f, 0.f, 0.f, 0.f};
+  if (active) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { g[i] = gamma[4 * q + i]; be[i] = beta[4 * q + i]; }
+  }
+  // xh and dyp of one position's 4 channels
+  auto load = [&](int p, float* xh, float* dyp) {
+    const float4 xv = ld4(xp + static_cast<long long>(p) * xs);
+    float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {                                    // constant indices keep srcs out of local memory
+      if (s < srcs.count) {
+        const float4 t = ld4(srcs.ptr[s] + (static_cast<long long>(n) * P + p) * srcs.stride[s] + 4 * q);
+        d.x += t.x; d.y += t.y; d.z += t.z; d.w += t.w;
+      }
+    }
+    const float xv4[4] = {xv.x, xv.y, xv.z, xv.w}, dv[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      xh[i] = (xv4[i] - m) * r;
+      dyp[i] = dv[i] * p_act_grad(g[i] * xh[i] + be[i], act, alpha);
+    }
+  };
+  float a = 0.f, b = 0.f;
+  float sg[4] = {0.f, 0.f, 0.f, 0.f}, sb[4] = {0.f, 0.f, 0.f, 0.f};
+  if (active) {
+#pragma unroll 2
+    for (int p = p0 + l; p < p1; p += lanes) {
+      float xh[4], dyp[4];
+      load(p, xh, dyp);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        sb[i] += dyp[i];
+        sg[i] += dyp[i] * xh[i];
+      }
+      const float gy0 = g[0] * dyp[0], gy1 = g[1] * dyp[1], gy2 = g[2] * dyp[2], gy3 = g[3] * dyp[3];
+      a += (gy0 + gy1) + (gy2 + gy3);
+      b += (gy0 * xh[0] + gy1 * xh[1]) + (gy2 * xh[2] + gy3 * xh[3]);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { s_ch[threadIdx.x * 8 + i] = sg[i]; s_ch[threadIdx.x * 8 + 4 + i] = sb[i]; }
+  __syncthreads();
+  float tg[4] = {0.f, 0.f, 0.f, 0.f}, tb[4] = {0.f, 0.f, 0.f, 0.f};   // C <= 4 * blockDim
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int j = threadIdx.x + k * blockDim.x, jq = j >> 2, ji = j & 3;
+    if (j < C)
+      for (int ll = 0; ll < lanes; ++ll) {
+        tg[k] += s_ch[(ll * c4 + jq) * 8 + ji];
+        tb[k] += s_ch[(ll * c4 + jq) * 8 + 4 + ji];
+      }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int j = threadIdx.x + k * blockDim.x;
+    if (j < C) { s_ch[j] = tg[k]; s_ch[C + j] = tb[k]; }
+  }
+  ln_reduce2(a, b, s_warp, s_part, s_tot, cs);                      // its cluster barrier also publishes the rows
+  if (rank == 0) {
+    for (int j = threadIdx.x; j < 2 * C; j += blockDim.x) {
+      float t = 0.f;
+      if (cs > 1) {
+        cg::cluster_group cluster = cg::this_cluster();
+        for (int rr = 0; rr < cs; ++rr) t += *cluster.map_shared_rank(s_ch + j, rr);
+      } else {
+        t = s_ch[j];
+      }
+      (j < C ? wg : wb)[static_cast<long long>(n) * C + (j < C ? j : j - C)] = t;
+    }
+  }
+  const float inv = 1.f / (static_cast<float>(P) * C);
+  const float mg = a * inv, mgx = b * inv;
+  if (active) {
+    float* dp = dx + static_cast<long long>(n) * P * dxs + 4 * q;
+#pragma unroll 2
+    for (int p = p0 + l; p < p1; p += lanes) {
+      float xh[4], dyp[4], o[4];
+      load(p, xh, dyp);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) o[i] = r * (g[i] * dyp[i] - mg - xh[i] * mgx);
+      *reinterpret_cast<float4*>(dp + static_cast<long long>(p) * dxs) = make_float4(o[0], o[1], o[2], o[3]);
+    }
+  }
+  if (cs > 1) cg::this_cluster().sync();
+}
+
 }  // namespace vp
+
+using namespace vp;
+
+extern "C" int vp_lnorm_act(const float* x, int x_cstride, float* y, int y_cstride, int n, int positions, int c, const float* gamma,
+                            const float* beta, float eps, int act, float alpha, float* stats, vp_stream_t stream) {
+  if (!x || !y) return set_error("vp_lnorm_act: null pointer");
+  if (n < 1 || positions < 1 || c < 4) return set_error("vp_lnorm_act: empty shape (n %d, positions %d, c %d)", n, positions, c);
+  if (c % 4 || x_cstride % 4 || y_cstride % 4 || x_cstride < c || y_cstride < c)
+    return set_error("vp_lnorm_act: channels/strides must be multiples of 4, strides >= channels");
+  LnPlan pl;
+  if (!plan_lnorm(positions, c, &pl)) return set_error("vp_lnorm_act: at most %d channels", 4 * kLnMaxThreads);
+  return launch_cluster(lnorm_act_kernel, dim3(pl.cs * n), pl.threads, 0, pl.cs, as_stream(stream), x, x_cstride, y, y_cstride, positions,
+                        c, gamma, beta, eps, act, alpha, stats, pl.lanes, pl.ppc, pl.cs);
+}
+
+extern "C" int vp_lnorm_act_bwd(const float* x, int x_cstride, const float* const* dy, const int* dy_cstride, int num_dy, float* dx,
+                                int dx_cstride, int n, int positions, int c, const float* gamma, const float* beta, const float* stats,
+                                int act, float alpha, float* dgamma, float* dbeta, vp_stream_t stream) {
+  if (!x || !dy || !dy_cstride || !dx || !stats || !gamma || !beta || !dgamma || !dbeta) return set_error("vp_lnorm_act_bwd: null pointer");
+  if (num_dy < 1 || num_dy > 4) return set_error("vp_lnorm_act_bwd: 1 to 4 gradient sources, got %d", num_dy);
+  if (n < 1 || positions < 1 || c < 4) return set_error("vp_lnorm_act_bwd: empty shape (n %d, positions %d, c %d)", n, positions, c);
+  bool ok = c % 4 == 0 && x_cstride % 4 == 0 && dx_cstride % 4 == 0 && x_cstride >= c && dx_cstride >= c;
+  for (int i = 0; i < num_dy; ++i) ok = ok && dy[i] && dy_cstride[i] % 4 == 0 && dy_cstride[i] >= c;
+  if (!ok) return set_error("vp_lnorm_act_bwd: null source, or channels/strides not multiples of 4 / strides below channels");
+  LnPlan pl;
+  if (!plan_lnorm(positions, c, &pl)) return set_error("vp_lnorm_act_bwd: at most %d channels", 4 * kLnMaxThreads);
+  SlabSrcs s;
+  s.count = num_dy;
+  for (int i = 0; i < 4; ++i) { s.ptr[i] = i < num_dy ? dy[i] : nullptr; s.stride[i] = i < num_dy ? dy_cstride[i] : 0; }
+  // per-sample partials of dgamma / dbeta (rows of the scratch buffer), added to the outputs in sample order
+  float* ws = nullptr;
+  if (scratch_alloc(&ws, 2LL * n * c, stream)) return -1;
+  float *wg = ws, *wb = ws + static_cast<long long>(n) * c;
+  int rc = launch_cluster(lnorm_act_bwd_kernel, dim3(n * pl.cs), pl.threads, static_cast<size_t>(pl.threads) * 8 * sizeof(float), pl.cs,
+                          as_stream(stream), x, x_cstride, s, dx, dx_cstride, positions, c, gamma, beta, stats, act, alpha, wg, wb,
+                          pl.lanes, pl.ppc, pl.cs);
+  if (rc == 0) rc = reduce_parts(wg, n, c, dgamma, stream);
+  if (rc == 0) rc = reduce_parts(wb, n, c, dbeta, stream);
+  scratch_free(ws, stream);
+  return rc;
+}

@@ -300,6 +300,12 @@ def inorm_act(x_addr, x_cs, y_addr, y_cs, n, positions, c, gamma, beta, act=ACT_
                              ptr(stats), stream_ptr()))
 
 
+def lnorm_act(x_addr, x_cs, y_addr, y_cs, n, positions, c, gamma, beta, act=ACT_NONE, alpha=0.0, stats=None, eps=1e-12):
+    """Layer norm over all positions and channels of each sample (vp_lnorm_act); stats [n, 2]."""
+    check(lib().vp_lnorm_act(C.c_void_p(x_addr), x_cs, C.c_void_p(y_addr), y_cs, n, positions, c, ptr(gamma), ptr(beta), _f(eps), act,
+                             _f(alpha), ptr(stats), stream_ptr()))
+
+
 def lstm_gates_fwd(pre, n, positions, filters, c_prev, g1, b1, g2, b2, c_new, h_dsts, stats1=None, stats2=None,
                    forget_bias=1.0, eps=1e-6):
     if 'gates' in _SKIP:
@@ -406,6 +412,12 @@ def inorm_act_bwd(x_addr, x_cs, dy_srcs, dx_addr, dx_cs, n, positions, c, gamma,
         return
     pa, sa, k = _srcs(dy_srcs)
     check(lib().vp_inorm_act_bwd(addr(x_addr), x_cs, pa, sa, k, addr(dx_addr), dx_cs, n, positions, c, ptr(gamma), ptr(beta),
+                                 ptr(stats), act, _f(alpha), ptr(dgamma), ptr(dbeta), stream_ptr()))
+
+
+def lnorm_act_bwd(x_addr, x_cs, dy_srcs, dx_addr, dx_cs, n, positions, c, gamma, beta, stats, act, alpha, dgamma, dbeta):
+    pa, sa, k = _srcs(dy_srcs)
+    check(lib().vp_lnorm_act_bwd(addr(x_addr), x_cs, pa, sa, k, addr(dx_addr), dx_cs, n, positions, c, ptr(gamma), ptr(beta),
                                  ptr(stats), act, _f(alpha), ptr(dgamma), ptr(dbeta), stream_ptr()))
 
 

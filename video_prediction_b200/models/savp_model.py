@@ -236,8 +236,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise ValueError('Unknown GAN loss type %s' % hp.gan_loss_type)                 # losses.py:52-53
         unsupported = []
         for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'),
-                          ('norm_layer', 'instance'), ('downsample_layer', 'conv_pool2d'),
+                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('downsample_layer', 'conv_pool2d'),
                           ('upsample_layer', 'upsample_conv2d'), ('activation_layer', 'relu'), ('last_frames', 1),
                           ('prev_image_background', True), ('first_image_background', True),
                           ('last_image_background', False), ('last_context_image_background', False),
@@ -249,6 +248,10 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             #  code of the reference reads it, base_model.py:90-95)
             if getattr(hp, key) != want:
                 unsupported.append('%s=%r' % (key, getattr(hp, key)))
+        # the normaliser of every convolution outside the ConvLSTM cells (savp_model.py:394, ops.py:1062-1073): instance,
+        # layer or none; 'batch' would need moving averages and a train / test switch
+        if hp.norm_layer not in ('instance', 'layer', 'none'):
+            unsupported.append('norm_layer=%r' % (hp.norm_layer,))
         # the ConvLSTM's normalisation (savp_model.py:370-390): instance norms inside the cell, none, or (ablation) one
         # instance norm on the cell's output
         if hp.conv_rnn_norm_layer not in ('instance', 'none'):
@@ -277,6 +280,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         """True: the reference's default ConvLSTM, with instance norms inside the cell.  False: the norm-free cell
         (conv_rnn_norm_layer='none', or the ablation_conv_rnn_norm form), whose gate math runs in the engine's epilogue."""
         return self.hparams.conv_rnn_norm_layer == 'instance' and not self.hparams.ablation_conv_rnn_norm
+
+    @property
+    def norm_scope(self):
+        """Variable scope of the normaliser at the norm_layer sites (h0.., the h_flow / h_scratch / h_masks heads, encoder
+        layers 2..): the default scope of the layer ops.get_norm_layer picks (ops.py:1062-1073), or None for
+        norm_layer='none' (tf.identity, no variables).  The ConvLSTM's own norms follow conv_rnn_norm_layer instead."""
+        return {'instance': 'InstanceNorm', 'layer': 'LayerNorm'}.get(self.hparams.norm_layer)
 
     # ------------------------------------------------------------------ structure (savp_model.py:182-232)
     @staticmethod
@@ -313,9 +323,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 oc = hp.nef * min(2 ** i, 4)
                 specs['%s/layer_%d/conv2d/kernel' % (sc, i + 1)] = ((4, 4, cin, oc), 'kernel')
                 specs['%s/layer_%d/conv2d/bias' % (sc, i + 1)] = ((oc,), 'zeros')
-                if i > 0:
-                    specs['%s/layer_%d/InstanceNorm/gamma' % (sc, i + 1)] = ((oc,), 'ones')
-                    specs['%s/layer_%d/InstanceNorm/beta' % (sc, i + 1)] = ((oc,), 'zeros')
+                if i > 0 and self.norm_scope:
+                    specs['%s/layer_%d/%s/gamma' % (sc, i + 1, self.norm_scope)] = ((oc,), 'ones')
+                    specs['%s/layer_%d/%s/beta' % (sc, i + 1, self.norm_scope)] = ((oc,), 'zeros')
                 cin = oc
             for nm in ('z_mu', 'z_log_sigma_sq'):
                 specs['%s/%s/dense/kernel' % (sc, nm)] = ((cin, hp.nz), 'kernel')
@@ -328,6 +338,10 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         def norm(name, c):
             specs[name + '/gamma'] = ((c,), 'ones')
             specs[name + '/beta'] = ((c,), 'zeros')
+
+        def site_norm(site, c):
+            if self.norm_scope:
+                norm('%s/%s' % (site, self.norm_scope), c)
 
         def lstm(i, cin, oc):
             b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, i)
@@ -345,7 +359,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             ks = 5 if i == 0 else 3
             specs['%s/h%d/conv_pool2d/kernel' % (sc, i)] = ((ks, ks, cin + Zc, oc), 'kernel')
             specs['%s/h%d/conv_pool2d/bias' % (sc, i)] = ((oc,), 'zeros')
-            norm('%s/h%d/InstanceNorm' % (sc, i), oc)
+            site_norm('%s/h%d' % (sc, i), oc)
             if use:
                 lstm(i, oc, oc)
             outs.append(oc)
@@ -356,7 +370,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             cin = outs[-1] if i == 0 else outs[-1] + outs[n_enc - i - 1]
             specs['%s/h%d/upsample_conv2d/kernel' % (sc, li)] = ((3, 3, cin + Zc, oc), 'kernel')
             specs['%s/h%d/upsample_conv2d/bias' % (sc, li)] = ((oc,), 'zeros')
-            norm('%s/h%d/InstanceNorm' % (sc, li), oc)
+            site_norm('%s/h%d' % (sc, li), oc)
             if use:
                 lstm(li, oc, oc)
             outs.append(oc)
@@ -369,7 +383,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if hp.transformation == 'flow':         # savp_model.py:522-530: flow heads instead of the CDNA kernel dense layer
             specs['%s/h%d_flow/conv2d/kernel' % (sc, nl)] = ((3, 3, top, hp.ngf), 'kernel')
             specs['%s/h%d_flow/conv2d/bias' % (sc, nl)] = ((hp.ngf,), 'zeros')
-            norm('%s/h%d_flow/InstanceNorm' % (sc, nl), hp.ngf)
+            site_norm('%s/h%d_flow' % (sc, nl), hp.ngf)
             specs[sc + '/flows/conv2d/kernel'] = ((3, 3, hp.ngf, 2 * nk), 'kernel')
             specs[sc + '/flows/conv2d/bias'] = ((2 * nk,), 'zeros')
         else:
@@ -378,7 +392,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         for nm in ('h%d_scratch' % nl, 'h%d_masks' % nl):
             specs['%s/%s/conv2d/kernel' % (sc, nm)] = ((3, 3, top, hp.ngf), 'kernel')
             specs['%s/%s/conv2d/bias' % (sc, nm)] = ((hp.ngf,), 'zeros')
-            norm('%s/%s/InstanceNorm' % (sc, nm), hp.ngf)
+            site_norm('%s/%s' % (sc, nm), hp.ngf)
         specs[sc + '/scratch_image/conv2d/kernel'] = ((3, 3, hp.ngf, C), 'kernel')
         specs[sc + '/scratch_image/conv2d/bias'] = ((C,), 'zeros')
         nlayers = nk + 3
@@ -680,6 +694,49 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
     def _z(self, *shape):
         return torch.zeros(*shape, device=self.device, dtype=torch.float32)
 
+    # ------------------------------------------------------------------ norm_layer sites (ops.get_norm_layer, ops.py:1062-1073)
+    # Each site is conv -> normaliser -> activation.  'instance' and 'layer' run the convolution into a `pre` buffer and
+    # the norm kernel from there into the site's output slice; 'none' has the convolution's epilogue apply bias +
+    # activation straight into that slice, and the backward takes the activation gradient from the output.
+    def _norm_stats(self, *lead_and_c):
+        """Per-call statistics of a site: [.., c, 2] (instance), [.., 2] (layer) or empty (none)."""
+        lead, c = lead_and_c[:-1], lead_and_c[-1]
+        return self._z(*lead, *{'instance': (c, 2), 'layer': (2,)}.get(self.hparams.norm_layer, (0,)))
+
+    def _site_conv(self, conv, x, pre, out, out_off=0, act=L.ACT_RELU, alpha=0.0):
+        if self.hparams.norm_layer == 'none':
+            conv.fwd(x, out, out_off=out_off, act=act, alpha=alpha)
+        else:
+            conv.fwd(x, pre)
+
+    def _site_norm(self, site, pre, out_addr, out_cs, n, positions, c, act, alpha, stats):
+        """out = act(norm(pre)) with the variables `site`/<norm_scope>; nothing to do for 'none'."""
+        if self.norm_scope is None:
+            return
+        nm = '%s/%s' % (site, self.norm_scope)
+        fn = L.inorm_act if self.hparams.norm_layer == 'instance' else L.lnorm_act
+        fn(pre.data_ptr(), c, out_addr, out_cs, n, positions, c, self.params[nm + '/gamma'], self.params[nm + '/beta'], act, alpha,
+           stats)
+
+    def _site_norm_bwd(self, site, pre, y_addr, y_cs, srcs, dpre, n, positions, c, act, alpha, stats):
+        """dpre from the gradient sources `srcs` (summed) of the site's output y (at y_addr); accumulates the norm's
+        gamma / beta gradients."""
+        if self.norm_scope is None:
+            rows, dp = n * positions, dpre.data_ptr()
+            if len(srcs) > 2:            # act_bwd adds two sources: fold the others into dpre first
+                L.axpy_channels(srcs[0][0], srcs[0][1], dp, c, rows, c, accumulate=False)
+                for a, cs in srcs[1:-1]:
+                    L.axpy_channels(a, cs, dp, c, rows, c)
+                srcs = [(dp, c), srcs[-1]]
+            b = srcs[1] if len(srcs) > 1 else (0, c)
+            L.act_bwd(y_addr, y_cs, srcs[0][0], srcs[0][1], b[0], b[1], dp, c, rows, c, act, alpha)
+            return
+        nm = '%s/%s' % (site, self.norm_scope)
+        fn = L.inorm_act_bwd if self.hparams.norm_layer == 'instance' else L.lnorm_act_bwd
+        P, Gp = self.params, self.grads
+        fn(pre.data_ptr(), c, srcs, dpre.data_ptr(), c, n, positions, c, P[nm + '/gamma'], P[nm + '/beta'], stats, act, alpha,
+           Gp[nm + '/gamma'], Gp[nm + '/beta'])
+
     def _build_generator(self):
         hp = self.hparams
         S, NB, H, W, C, Zc = self.S, self.NB, self.H, self.W, self.C, self.Zc
@@ -720,7 +777,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                                       (0, 2, 2), True, d['in_spec'], oc)
             self.convs.append(d['conv'])
             Bf['pre%d' % li] = self._z(S, NB, hh, ww, oc)
-            Bf['nst%d' % li] = self._z(S, NB, oc, 2)
+            Bf['nst%d' % li] = self._norm_stats(S, NB, oc)
             if use:
                 d['rin_spec'] = ConcatSpec([('x', oc)] + zseg + [('h', oc)])
                 Bf['rin%d' % li] = self._z(S + 1, NB, hh, ww, d['rin_spec'].cstride)
@@ -775,13 +832,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                                         (1, 1, 1), (0, 1, 1), False, hs_spec, 2 * nk)
             self.convs += [self.conv_hflow, self.conv_flows]
             Bf['fpre'] = self._z(S, NB, H, W, hp.ngf)
-            Bf['fst'] = self._z(S, NB, hp.ngf, 2)
+            Bf['fst'] = self._norm_stats(S, NB, hp.ngf)
             Bf['hf'] = self._z(S, NB, H, W, hp.ngf)
             Bf['flows'] = self._z(S, NB, H, W, _ceil4(2 * nk))
         Bf['spre'] = self._z(S, NB, H, W, hp.ngf)
         Bf['mpre'] = self._z(S, NB, H, W, hp.ngf)
-        Bf['sst'] = self._z(S, NB, hp.ngf, 2)
-        Bf['mst'] = self._z(S, NB, hp.ngf, 2)
+        Bf['sst'] = self._norm_stats(S, NB, hp.ngf)
+        Bf['mst'] = self._norm_stats(S, NB, hp.ngf)
         Bf['hs'] = self._z(S, NB, H, W, hp.ngf)
         Bf['mk'] = self._z(S, NB, H, W, self.mk_spec.cstride)
         Bf['mlog'] = self._z(S, NB, H, W, 8)
@@ -834,7 +891,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['epre%d' % i] = self._z(S * B, hh, ww, oc)
             if i > 0:
                 Bf['eact%d' % i] = self._z(S * B, hh, ww, oc)
-                Bf['est%d' % i] = self._z(S * B, oc, 2)
+                Bf['est%d' % i] = self._norm_stats(S * B, oc)
             self.enc_layers.append(dict(conv=conv, oc=oc, h=hh, w=ww))
             spec = ConcatSpec([('x', oc)])
         Bf['epool'] = self._z(S * B, self.enc_layers[-1]['oc'])
@@ -1024,12 +1081,11 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 el['conv'].fwd(cur, pre, act=L.ACT_LRELU, alpha=0.2)      # networks.py:17-20
                 cur = pre
             else:
-                el['conv'].fwd(cur, pre)
-                nm = 'generator/encoder/layer_%d/InstanceNorm' % (i + 1)
-                L.inorm_act(pre.data_ptr(), el['oc'], Bf['eact%d' % i].data_ptr(), el['oc'], S * B, el['h'] * el['w'],
-                            el['oc'], self.params[nm + '/gamma'], self.params[nm + '/beta'], L.ACT_LRELU, 0.2,
-                            Bf['est%d' % i])
-                cur = Bf['eact%d' % i]
+                out = Bf['eact%d' % i]
+                self._site_conv(el['conv'], cur, pre, out, act=L.ACT_LRELU, alpha=0.2)
+                self._site_norm('generator/encoder/layer_%d' % (i + 1), pre, out.data_ptr(), el['oc'], S * B, el['h'] * el['w'],
+                                el['oc'], L.ACT_LRELU, 0.2, Bf['est%d' % i])
+                cur = out
         last = self.enc_layers[-1]
         L.avgpool(cur, last['oc'], Bf['epool'], S * B, last['h'] * last['w'], last['oc'])
         P = self.params
@@ -1128,13 +1184,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         for d in self.gl:
             li, oc, hh, ww = d['li'], d['oc'], d['h'], d['w']
             pre = Bf['pre%d' % li][t]
-            d['conv'].fwd(Bf['in%d' % li][t], pre)
-            nm = '%s/h%d/InstanceNorm' % (sc, li)
+            site = '%s/h%d' % (sc, li)
             if d['use']:
                 rsp = d['rin_spec']
                 rin = Bf['rin%d' % li][t]
-                L.inorm_act(pre.data_ptr(), oc, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc,
-                            P[nm + '/gamma'], P[nm + '/beta'], L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
+                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, rin, rsp.off('x'))
+                self._site_norm(site, pre, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc, L.ACT_RELU, 0.0,
+                                Bf['nst%d' % li][t])
                 gpre = Bf['gpre%d' % li][t]
                 b = d['rname']
                 if self.cell_norm:
@@ -1157,8 +1213,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             else:
                 dests = self._h_dests(li, t)
                 out = Bf['out%d' % li][t]
-                L.inorm_act(pre.data_ptr(), oc, out.data_ptr(), oc, NB, hh * ww, oc, P[nm + '/gamma'], P[nm + '/beta'],
-                            L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
+                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, out)
+                self._site_norm(site, pre, out.data_ptr(), oc, NB, hh * ww, oc, L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
                 for addr, cs in dests:
                     L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
         nk, kh, kw = self.nk, self.kh, self.kw
@@ -1167,10 +1223,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         nl = self.nl
         if self.flow:
             # flow heads (savp_model.py:522-530): h_flow = relu(IN(conv3x3(top))), flows = conv3x3(h_flow) [.., 2, nk]
-            self.conv_hflow.fwd(top, Bf['fpre'][t])
-            nm = '%s/h%d_flow/InstanceNorm' % (sc, nl)
-            L.inorm_act(Bf['fpre'][t].data_ptr(), ngf, Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, P[nm + '/gamma'], P[nm + '/beta'],
-                        L.ACT_RELU, 0.0, Bf['fst'][t])
+            self._site_conv(self.conv_hflow, top, Bf['fpre'][t], Bf['hf'][t])
+            self._site_norm('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, L.ACT_RELU, 0.0,
+                            Bf['fst'][t])
             self.conv_flows.fwd(Bf['hf'][t], Bf['flows'][t], out_c=2 * nk)
         else:
             # cdna kernels (savp_model.py:546-559)
@@ -1181,16 +1236,14 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                         kh * kw * nk, NB, K, kh * kw * nk, k_splits=32)
             L.cdna_kernel_norm(Bf['kraw'][t], Bf['kern'][t], NB, kh, kw, nk)
         # heads
-        self.conv_scratch.fwd(top, Bf['spre'][t])
-        self.conv_hmasks.fwd(top, Bf['mpre'][t])
-        nm = '%s/h%d_scratch/InstanceNorm' % (sc, nl)
-        L.inorm_act(Bf['spre'][t].data_ptr(), ngf, Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, P[nm + '/gamma'],
-                    P[nm + '/beta'], L.ACT_RELU, 0.0, Bf['sst'][t])
         mk = Bf['mk'][t]
         msp = self.mk_spec
-        nm = '%s/h%d_masks/InstanceNorm' % (sc, nl)
-        L.inorm_act(Bf['mpre'][t].data_ptr(), ngf, mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
-                    P[nm + '/gamma'], P[nm + '/beta'], L.ACT_RELU, 0.0, Bf['mst'][t])
+        self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t])
+        self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'))
+        self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, L.ACT_RELU, 0.0,
+                        Bf['sst'][t])
+        self._site_norm('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
+                        L.ACT_RELU, 0.0, Bf['mst'][t])
         # scratch image -> last layer slot (savp_model.py:570-572, 595-596)
         self.conv_simg.fwd(Bf['hs'][t], mk, out_off=msp.off('l%d' % (self.nlayers - 1)), out_c=C, act=L.ACT_SIGMOID)
         # transformed images: 4 CDNA (or flow-warped) + prev image + first image (savp_model.py:574-584)

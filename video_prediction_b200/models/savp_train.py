@@ -336,19 +336,17 @@ class TrainMixin(object):
                         G['dlay'][t], 4 * nlay, NB * HW, nlay)
         self.conv_masks.dgrad(G['dmlog'][t], dmk, dy_c=nlay)
         # h_masks branch
-        nm = '%s/h%d_masks/InstanceNorm' % (sc, nl)
-        L.inorm_act_bwd(Bf['mpre'][t].data_ptr(), ngf, [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t].data_ptr(),
-                        ngf, NB, HW, ngf, P[nm + '/gamma'], P[nm + '/beta'], Bf['mst'][t], L.ACT_RELU, 0.0, Gp[nm + '/gamma'],
-                        Gp[nm + '/beta'])
+        self._site_norm_bwd('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride,
+                            [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, L.ACT_RELU, 0.0,
+                            Bf['mst'][t])
         self.conv_hmasks.dgrad(G['dmpre'][t], G['dtop'][t])
         # scratch branch
         so = msp.off('l%d' % (nlay - 1))
         L.act_bwd(mk.data_ptr() + 4 * so, msp.cstride, dmk.data_ptr() + 4 * so, msp.cstride,
                   G['dlay'][t].data_ptr() + 4 * 4 * (nlay - 1), 4 * nlay, G['dsimg'][t].data_ptr(), 4, NB * HW, C, L.ACT_SIGMOID)
         self.conv_simg.dgrad(G['dsimg'][t], G['dhs'][t], dy_c=C)
-        nm = '%s/h%d_scratch/InstanceNorm' % (sc, nl)
-        L.inorm_act_bwd(Bf['spre'][t].data_ptr(), ngf, [(G['dhs'][t].data_ptr(), ngf)], G['dspre'][t].data_ptr(), ngf, NB, HW, ngf,
-                        P[nm + '/gamma'], P[nm + '/beta'], Bf['sst'][t], L.ACT_RELU, 0.0, Gp[nm + '/gamma'], Gp[nm + '/beta'])
+        self._site_norm_bwd('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, [(G['dhs'][t].data_ptr(), ngf)],
+                            G['dspre'][t], NB, HW, ngf, L.ACT_RELU, 0.0, Bf['sst'][t])
         self.conv_scratch.dgrad(G['dspre'][t], G['dtop'][t], accumulate=True)
         nk, kh, kw = self.nk, self.kh, self.kw
         G['dimg'][t].zero_()
@@ -357,9 +355,8 @@ class TrainMixin(object):
             L.flow_apply_bwd(Bf['img'][t], Bf['flows'][t], Bf['flows'].shape[-1], dmk.data_ptr() + 4 * msp.off('l0'), msp.cstride,
                              G['dlay'][t].data_ptr(), 4 * nlay, G['dimg'][t], G['dflows'][t], NB, H, W, nk)
             self.conv_flows.dgrad(G['dflows'][t], G['dhf'][t], dy_c=2 * nk)
-            nm = '%s/h%d_flow/InstanceNorm' % (sc, nl)
-            L.inorm_act_bwd(Bf['fpre'][t].data_ptr(), ngf, [(G['dhf'][t].data_ptr(), ngf)], G['dfpre'][t].data_ptr(), ngf, NB, HW, ngf,
-                            P[nm + '/gamma'], P[nm + '/beta'], Bf['fst'][t], L.ACT_RELU, 0.0, Gp[nm + '/gamma'], Gp[nm + '/beta'])
+            self._site_norm_bwd('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, [(G['dhf'][t].data_ptr(), ngf)],
+                                G['dfpre'][t], NB, HW, ngf, L.ACT_RELU, 0.0, Bf['fst'][t])
             self.conv_hflow.dgrad(G['dfpre'][t], G['dtop'][t], accumulate=True)
         else:
             # CDNA
@@ -389,7 +386,6 @@ class TrainMixin(object):
                 srcs.append((G['din%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
             if li == n_enc - 1 and not self.flow:
                 srcs.append((G['dsmall'][t].data_ptr(), oc))
-            nm = '%s/h%d/InstanceNorm' % (sc, li)
             if d['use'] and not self.cell_norm:
                 rsp = d['rin_spec']
                 if 'hst%d' % li in Bf:    # h -> IN(h) -> consumers: their gradient through the norm, before the recurrent one
@@ -417,9 +413,12 @@ class TrainMixin(object):
                                  Gp[b + '/state/gamma'], Gp[b + '/state/beta'])
                 d['rconv'].dgrad(G['dgpre%d' % li][t], G['drin%d' % li][t])
                 srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
-            L.inorm_act_bwd(Bf['pre%d' % li][t].data_ptr(), oc, srcs, G['dpre%d' % li][t].data_ptr(), oc, NB, hh * ww, oc,
-                            P[nm + '/gamma'], P[nm + '/beta'], Bf['nst%d' % li][t], L.ACT_RELU, 0.0, Gp[nm + '/gamma'],
-                            Gp[nm + '/beta'])
+            if d['use']:         # the site's output: the 'x' slot of the ConvLSTM's input, or the layer's own buffer
+                y_addr, y_cs = Bf['rin%d' % li][t].data_ptr() + 4 * d['rin_spec'].off('x'), d['rin_spec'].cstride
+            else:
+                y_addr, y_cs = Bf['out%d' % li][t].data_ptr(), oc
+            self._site_norm_bwd('%s/h%d' % (sc, li), Bf['pre%d' % li][t], y_addr, y_cs, srcs, G['dpre%d' % li][t], NB, hh * ww, oc,
+                                L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
             d['conv'].dgrad(G['dpre%d' % li][t], G['din%d' % li][t])
         # gradient w.r.t. the input image of this step: CDNA path + first conv's 'image' slot
         sp = self.gl[0]['in_spec']
@@ -530,10 +529,9 @@ class TrainMixin(object):
                 dact = G['deact%d' % i] if i > 0 else G['depre0']
                 L.avgpool_bwd(G['depool'], dact, oc, S * B, pos, oc)
             if i > 0:
-                nm = '%s/layer_%d/InstanceNorm' % (sc, i + 1)
-                L.inorm_act_bwd(Bf['epre%d' % i].data_ptr(), oc, [(G['deact%d' % i].data_ptr(), oc)], G['depre%d' % i].data_ptr(), oc,
-                                S * B, pos, oc, P[nm + '/gamma'], P[nm + '/beta'], Bf['est%d' % i], L.ACT_LRELU, 0.2,
-                                Gp[nm + '/gamma'], Gp[nm + '/beta'])
+                self._site_norm_bwd('%s/layer_%d' % (sc, i + 1), Bf['epre%d' % i], Bf['eact%d' % i].data_ptr(), oc,
+                                    [(G['deact%d' % i].data_ptr(), oc)], G['depre%d' % i], S * B, pos, oc, L.ACT_LRELU, 0.2,
+                                    Bf['est%d' % i])
                 x_in = Bf['eact%d' % (i - 1)] if i > 1 else Bf['epre0']
                 dst = G['deact%d' % (i - 1)] if i > 1 else G['depre0']
                 el['conv'].dgrad(G['depre%d' % i], dst)

@@ -45,8 +45,10 @@ typedef struct vp_conv_geom {
   int32_t transposed;
 } vp_conv_geom;
 
-enum { VP_ACT_NONE = 0, VP_ACT_RELU = 1, VP_ACT_LRELU = 2, VP_ACT_SIGMOID = 3, VP_ACT_TANH = 4 };
-enum { VP_WKIND_PLAIN = 0, VP_WKIND_POOLED = 1, VP_WKIND_UPSAMPLED = 2 };
+/* VP_ACT_ELU: tf.nn.elu, x for x > 0 and exp(x) - 1 otherwise.  Every fused activation (the engine epilogue and
+ * vp_conv_igemm_actgrad, vp_act_bwd, vp_inorm_act(_bwd), vp_lnorm_act(_bwd)) takes NONE .. ELU; other values are an error. */
+enum { VP_ACT_NONE = 0, VP_ACT_RELU = 1, VP_ACT_LRELU = 2, VP_ACT_SIGMOID = 3, VP_ACT_TANH = 4, VP_ACT_ELU = 5 };
+enum { VP_WKIND_PLAIN = 0, VP_WKIND_POOLED = 1, VP_WKIND_UPSAMPLED = 2, VP_WKIND_DECONV = 3 };
 enum { VP_WLAYOUT_FWD = 0, VP_WLAYOUT_DGRAD = 1,
        VP_WLAYOUT_RESIDUAL = 4 /* OR-ed in: pack tf32(w - tf32(w)), the low part of the fp32-exact 3xTF32 mode */,
        VP_WLAYOUT_GATES = 8    /* OR-ed in (FWD only, co = 4F, F % 32 == 0): GEMM column 128 t + 32 g + c holds gate g
@@ -70,7 +72,7 @@ int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const float* wpack
                   vp_stream_t stream);
 
 /* Input-gradient convolution fused with the backward of the previous layer's activation:
- *   out = (conv(in) + addend) * act'(act_output),  act' evaluated from the activation OUTPUT (lrelu/relu/sigmoid/tanh);
+ *   out = (conv(in) + addend) * act'(act_output),  act' evaluated from the activation OUTPUT (any VP_ACT_*);
  * act_output / addend (optional) have exactly the layout of the dense `out`.  Used for the discriminator towers
  * (lrelu(conv3d), networks.py:83-102), where it removes one full read+write pass per layer. */
 int vp_conv_igemm_actgrad(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
@@ -106,6 +108,8 @@ int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g
  *  kind PLAIN:     taps = kd*kh*kw, Keff = w
  *  kind POOLED:    2-D only, taps = (kh+1)*(kw+1): avg-pool(2x2,s1,FULL) of the kernel (ops.py:838-842)
  *  kind UPSAMPLED: 2-D only, taps = (kh+3)*(kw+3): bilinear (x) kernel (ops.py:698-704)
+ *  kind DECONV:    taps = kd*kh*kw, w in the conv2d_transpose layout [kd][kh][kw][co][ci_ref] (ops.py:567), Keff = w
+ *                  with its two channel axes swapped; vp_unpack_wgrad writes dw in the same layout
  *  layout FWD:   wpacked[tap][co (n_pad)][ci_int (kc*32)]
  *  layout DGRAD: wpacked[tap][ci_int (n_pad)][co (kc*32)]
  * cmap[ci_int] = reference input channel feeding internal channel ci_int, or -1 (zero column);

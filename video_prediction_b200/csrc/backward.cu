@@ -4,6 +4,7 @@
 // (BPTT sums over timesteps, savp_model.py unrolls share variables).
 #include <cstdint>
 
+#include "act.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -32,13 +33,6 @@ __device__ __forceinline__ void bsum(float* vals, float* scratch) {
     vals[i] = wsum(v);
   }
 }
-__device__ __forceinline__ float act_grad(float yp, int act, float alpha) {  // d act(yp) / d yp
-  switch (act) {
-    case VP_ACT_RELU: return yp > 0.f ? 1.f : 0.f;
-    case VP_ACT_LRELU: return yp > 0.f ? 1.f : alpha;
-    default: return 1.f;
-  }
-}
 
 struct SrcList {  // up to 4 gradient sources that are summed (each a channel slice with its own stride)
   const float* ptr[4];
@@ -50,6 +44,7 @@ struct SrcList {  // up to 4 gradient sources that are summed (each a channel sl
 // instance norm (+act) backward.  x: pre-norm input (dense, stride xs); dy: sum of `srcs`.
 // dx = r*(dxh - mean(dxh) - xh*mean(dxh*xh)),  dxh = dyp*gamma,  dyp = dy*act'(gamma*xh+beta)
 // ------------------------------------------------------------------------------------------------
+template <bool kElu>
 __global__ void __launch_bounds__(512) inorm_act_bwd_kernel(const float* __restrict__ x, int xs, SrcList srcs,
                                                             float* __restrict__ dx, int dxs, int P, int C,
                                                             const float* __restrict__ gamma,
@@ -87,7 +82,7 @@ __global__ void __launch_bounds__(512) inorm_act_bwd_kernel(const float* __restr
     const float dv[4] = {dy.x, dy.y, dy.z, dy.w};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const float dyp = dv[i] * act_grad(g[i] * xh[i] + b[i], act, alpha);
+      const float dyp = dv[i] * act_grad_pre<kElu>(g[i] * xh[i] + b[i], act, alpha);
       s[i] += dyp;
       s[4 + i] += dyp * xh[i];
     }
@@ -108,7 +103,7 @@ __global__ void __launch_bounds__(512) inorm_act_bwd_kernel(const float* __restr
     float o[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const float dyp = dv[i] * act_grad(g[i] * xh[i] + b[i], act, alpha);
+      const float dyp = dv[i] * act_grad_pre<kElu>(g[i] * xh[i] + b[i], act, alpha);
       // dxh = dyp*g ; mean(dxh) = g*s[i]/P ; mean(dxh*xh) = g*s[4+i]/P
       o[i] = r[i] * g[i] * (dyp - s[i] * inv - xh[i] * s[4 + i] * inv);
     }
@@ -662,6 +657,7 @@ __global__ void axpy_channels_kernel(const float* __restrict__ src, int ss, floa
   *o = accumulate ? *o + v : v;
 }
 // dy_pre = dy * act'(y)  from the activation OUTPUT y (sigmoid: y(1-y); lrelu/relu: sign of y)
+template <bool kElu>
 __global__ void act_bwd_from_output_kernel(const float* __restrict__ y, int ys, const float* __restrict__ dyA, int das,
                                            const float* __restrict__ dyB, int dbs, float* __restrict__ dx, int dxs,
                                            long long total, int C, int act, float alpha) {
@@ -671,11 +667,7 @@ __global__ void act_bwd_from_output_kernel(const float* __restrict__ y, int ys, 
   const long long r = idx / C;
   const float yv = y[r * ys + c];
   float d = dyA[r * das + c] + (dyB ? dyB[r * dbs + c] : 0.f);
-  if (act == VP_ACT_SIGMOID) d *= yv * (1.f - yv);
-  else if (act == VP_ACT_RELU) d = yv > 0.f ? d : 0.f;
-  else if (act == VP_ACT_LRELU) d = yv > 0.f ? d : alpha * d;
-  else if (act == VP_ACT_TANH) d *= (1.f - yv * yv);
-  dx[r * dxs + c] = d;
+  dx[r * dxs + c] = act_grad_mul<kElu>(d, yv, act, alpha);
 }
 // avg-pool backward: dx[n][p][c] = dy[n][c] / P
 __global__ void avgpool_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int dxs, long long total, int P, int C) {
@@ -890,6 +882,7 @@ extern "C" int vp_inorm_act_bwd(const float* x, int x_cstride, const float* cons
                                 const float* stats, int act, float alpha, float* dgamma, float* dbeta, vp_stream_t stream) {
   if (!x || !dy || !dx || !stats || !gamma || !beta || !dgamma || !dbeta) return set_error("vp_inorm_act_bwd: null pointer");
   if (c % 4 || num_dy < 1 || num_dy > 4) return set_error("vp_inorm_act_bwd: bad channel count / source count");
+  if (check_act(act, "vp_inorm_act_bwd")) return -1;
   {
     const int rc = slab_inorm_act_bwd(x, x_cstride, dy, dy_cstride, num_dy, dx, dx_cstride, n, positions, c, gamma, beta, stats, act, alpha,
                                       dgamma, dbeta, stream);
@@ -899,12 +892,13 @@ extern "C" int vp_inorm_act_bwd(const float* x, int x_cstride, const float* cons
   const int staged = positions <= 4096 ? 1 : 0;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(inorm_act_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4096 * 16);
+    cudaFuncSetAttribute(inorm_act_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4096 * 16);
+    cudaFuncSetAttribute(inorm_act_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4096 * 16);
     attr_set = true;
   }
   float* ws = nullptr;
   if (scratch_alloc(&ws, 2LL * n * c, stream)) return -1;
-  inorm_act_bwd_kernel<<<grid, positions >= 2048 ? 512 : 256, staged ? static_cast<size_t>(positions) * 32 : 0, as_stream(stream)>>>(
+  (act == VP_ACT_ELU ? inorm_act_bwd_kernel<true> : inorm_act_bwd_kernel<false>)<<<grid, positions >= 2048 ? 512 : 256, staged ? static_cast<size_t>(positions) * 32 : 0, as_stream(stream)>>>(
       x, x_cstride, make_srcs(dy, dy_cstride, num_dy), dx, dx_cstride, positions, c, gamma, beta, stats, act, alpha, ws,
       ws + static_cast<long long>(n) * c, staged);
   int rc = check_launch("inorm_act_bwd_kernel");
@@ -1058,8 +1052,9 @@ extern "C" int vp_axpy_channels(const float* src, int src_cstride, float* dst, i
 
 extern "C" int vp_act_bwd(const float* y, int y_cstride, const float* dy_a, int dy_a_cstride, const float* dy_b, int dy_b_cstride,
                           float* dx, int dx_cstride, long long rows, int c, int act, float alpha, vp_stream_t stream) {
+  if (check_act(act, "vp_act_bwd")) return -1;
   const long long total = rows * c;
-  act_bwd_from_output_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(y, y_cstride, dy_a, dy_a_cstride, dy_b,
+  (act == VP_ACT_ELU ? act_bwd_from_output_kernel<true> : act_bwd_from_output_kernel<false>)<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(y, y_cstride, dy_a, dy_a_cstride, dy_b,
                                                                                  dy_b_cstride, dx, dx_cstride, total, c, act, alpha);
   return check_launch("act_bwd_from_output_kernel");
 }

@@ -16,6 +16,11 @@ inline int check_launch(const char* what) {
   if (e != cudaSuccess) return set_error("%s launch failed: %s", what, cudaGetErrorString(e));
   return 0;
 }
+// Every fused activation takes VP_ACT_NONE .. VP_ACT_ELU.
+inline int check_act(int act, const char* what) {
+  if (act < VP_ACT_NONE || act > VP_ACT_ELU) return set_error("%s: unknown activation %d", what, act);
+  return 0;
+}
 inline cudaStream_t as_stream(vp_stream_t s) { return static_cast<cudaStream_t>(s); }
 // Sums that many blocks contribute to are made independent of block scheduling: every block writes its partial into its own
 // row of a stream-ordered scratch buffer (cudaMallocAsync, also valid inside a CUDA-graph capture) and reduce_parts adds

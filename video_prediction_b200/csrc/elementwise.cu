@@ -2,20 +2,12 @@
 // CDNA kernel head / apply, mask softmax + compositing, small utilities.
 // All tensors fp32 channels-last with an explicit channel stride so producers write straight into
 // the concat buffers their consumers read (no tf.concat / tile_concat materialisation passes).
+#include "act.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
 namespace vp {
 
-__device__ __forceinline__ float act_fn(float v, int act, float alpha) {
-  switch (act) {
-    case VP_ACT_RELU: return fmaxf(v, 0.f);
-    case VP_ACT_LRELU: return fmaxf(alpha * v, v);
-    case VP_ACT_SIGMOID: return 1.f / (1.f + __expf(-v));
-    case VP_ACT_TANH: return tanhf(v);
-    default: return v;
-  }
-}
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + __expf(-v)); }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -48,6 +40,7 @@ __device__ __forceinline__ void block_sum(float* vals, float* scratch) {
 // One CTA per (sample, group of 4 channels); three passes over a plane that lives in L2.
 // ------------------------------------------------------------------------------------------------
 // The (sample, 4-channel) plane is staged once in shared memory (16 B per position): one HBM/L2 read, one write.
+template <bool kElu>
 __global__ void __launch_bounds__(512) inorm_act_kernel(const float* __restrict__ x, int xs, float* __restrict__ y,
                                                         int ys, int P, int C, const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, float eps, int act,
@@ -87,8 +80,8 @@ __global__ void __launch_bounds__(512) inorm_act_kernel(const float* __restrict_
   for (int p = threadIdx.x; p < P; p += blockDim.x) {
     const float4 v = staged ? splane[p] : *reinterpret_cast<const float4*>(xp + static_cast<long long>(p) * xs);
     float4 o;
-    o.x = act_fn(v.x * g[0] + b[0], act, alpha); o.y = act_fn(v.y * g[1] + b[1], act, alpha);
-    o.z = act_fn(v.z * g[2] + b[2], act, alpha); o.w = act_fn(v.w * g[3] + b[3], act, alpha);
+    o.x = act_fwd<kElu>(v.x * g[0] + b[0], act, alpha); o.y = act_fwd<kElu>(v.y * g[1] + b[1], act, alpha);
+    o.z = act_fwd<kElu>(v.z * g[2] + b[2], act, alpha); o.w = act_fwd<kElu>(v.w * g[3] + b[3], act, alpha);
     *reinterpret_cast<float4*>(yp + static_cast<long long>(p) * ys) = o;
   }
 }
@@ -473,6 +466,7 @@ extern "C" int vp_inorm_act(const float* x, int x_cstride, float* y, int y_cstri
                             vp_stream_t stream) {
   if (!x || !y) return set_error("vp_inorm_act: null pointer");
   if (c % 4 || x_cstride % 4 || y_cstride % 4) return set_error("vp_inorm_act: channels/strides must be multiples of 4");
+  if (check_act(act, "vp_inorm_act")) return -1;
   {
     const int rc = slab_inorm_act(x, x_cstride, y, y_cstride, n, positions, c, gamma, beta, eps, act, alpha, stats, stream);
     if (rc <= 0) return rc;
@@ -482,10 +476,11 @@ extern "C" int vp_inorm_act(const float* x, int x_cstride, float* y, int y_cstri
   const size_t smem = staged ? static_cast<size_t>(positions) * 16 : 0;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(inorm_act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 16);
+    cudaFuncSetAttribute(inorm_act_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 16);
+    cudaFuncSetAttribute(inorm_act_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4096 * 16);
     attr_set = true;
   }
-  inorm_act_kernel<<<grid, positions >= 2048 ? 512 : 256, smem, as_stream(stream)>>>(x, x_cstride, y, y_cstride, positions, c, gamma, beta, eps, act,
+  (act == VP_ACT_ELU ? inorm_act_kernel<true> : inorm_act_kernel<false>)<<<grid, positions >= 2048 ? 512 : 256, smem, as_stream(stream)>>>(x, x_cstride, y, y_cstride, positions, c, gamma, beta, eps, act,
                                                            alpha, stats, staged);
   return check_launch("inorm_act_kernel");
 }

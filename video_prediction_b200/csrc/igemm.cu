@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "act.cuh"
 #include "common.h"
 #include "ptx.cuh"
 #include "tensormap.h"
@@ -72,31 +73,19 @@ struct alignas(64) IgemmArgs {
   Tap taps[kMaxTaps];
 };
 
-__device__ __forceinline__ float apply_act(float v, int act, float alpha) {
-  switch (act) {
-    case VP_ACT_RELU: return fmaxf(v, 0.f);
-    case VP_ACT_LRELU: return fmaxf(alpha * v, v);
-    case VP_ACT_SIGMOID: return 1.f / (1.f + __expf(-v));
-    case VP_ACT_TANH: return tanhf(v);
-    default: return v;
-  }
-}
-
 // Epilogue of one accumulator element: output element `ooff + col` of a valid row.
+template <bool kElu>
 __device__ __forceinline__ void fwd_store(const IgemmArgs& a, long long ooff, int col, float v, bool add_bias) {
   if (col >= a.out_c) return;
   float* o = a.out + ooff + col;
   if (a.accumulate == 2) v += *o;      // last pass of a multi-pass accumulation: the partial sum is added BEFORE bias / activation
   if (add_bias) v += __ldg(a.bias + col);
   if (a.splits > 1) { atomicAdd(o, v); return; }
-  v = apply_act(v, a.act, a.alpha);
+  v = act_fwd<kElu>(v, a.act, a.alpha);
   if (a.aux_y != nullptr) {            // fused backward of the previous layer's activation: (v + add) * act'(y)
     const float yv = __ldg(a.aux_y + ooff + col);
     if (a.aux_add != nullptr) v += __ldg(a.aux_add + ooff + col);
-    if (a.aux_act == VP_ACT_LRELU) v = yv > 0.f ? v : a.alpha * v;
-    else if (a.aux_act == VP_ACT_RELU) v = yv > 0.f ? v : 0.f;
-    else if (a.aux_act == VP_ACT_SIGMOID) v *= yv * (1.f - yv);
-    else if (a.aux_act == VP_ACT_TANH) v *= (1.f - yv * yv);
+    v = act_grad_mul<kElu>(v, yv, a.aux_act, a.alpha);
   }
   *o = a.accumulate == 1 ? *o + v : v;
 }
@@ -147,7 +136,7 @@ __device__ __forceinline__ void lstm_store(const IgemmArgs& a, long long pix, co
 // and a BN x 128 B weight tile, both 128B-swizzled.
 // ------------------------------------------------------------------------------------------------
 constexpr int kFwdThreads = 384;
-template <int BN, bool kLstm>
+template <int BN, bool kLstm, bool kElu = false>
 __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_constant__ IgemmArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -272,8 +261,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
           const int col = n0 + 8 * i + 2 * (lane & 3);
-          fwd_store(a, ooff, col, acc[4 * i + 2 * r], add_bias);
-          fwd_store(a, ooff, col + 1, acc[4 * i + 2 * r + 1], add_bias);
+          fwd_store<kElu>(a, ooff, col, acc[4 * i + 2 * r], add_bias);
+          fwd_store<kElu>(a, ooff, col + 1, acc[4 * i + 2 * r + 1], add_bias);
         }
       }
     }
@@ -632,6 +621,7 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
   if (kc < 1 || kc * 32 < in->c) return set_error("vp_conv_igemm: kc*32 must cover in->c");
   if (out->c > n_pad) return set_error("vp_conv_igemm: out->c exceeds n_pad");
   if (in->n != out->n) return set_error("vp_conv_igemm: batch mismatch");
+  if (check_act(act, "vp_conv_igemm") || check_act(aux_act, "vp_conv_igemm_actgrad")) return -1;
   if (split_k > 1 && act != VP_ACT_NONE) return set_error("vp_conv_igemm: split_k needs act NONE");
   if (aux_y && split_k > 1) return set_error("vp_conv_igemm: the fused activation gradient needs split_k <= 1");
   if (accumulate < 0 || accumulate > 2) return set_error("vp_conv_igemm: accumulate must be 0, 1 or 2 (got %d)", accumulate);
@@ -696,8 +686,9 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
   A.stages = static_cast<int>(std::min<size_t>(kMaxStagesFwd, (smem_max - 1024) / stage_bytes));
   const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
   typedef void (*FwdKernel)(const IgemmArgs);
-  static const FwdKernel kernels[4] = {igemm_fwd_kernel<32, false>, igemm_fwd_kernel<64, false>, igemm_fwd_kernel<128, false>,
-                                       igemm_fwd_kernel<128, true>};
+  static const FwdKernel kernels[7] = {igemm_fwd_kernel<32, false>, igemm_fwd_kernel<64, false>, igemm_fwd_kernel<128, false>,
+                                       igemm_fwd_kernel<128, true>, igemm_fwd_kernel<32, false, true>,
+                                       igemm_fwd_kernel<64, false, true>, igemm_fwd_kernel<128, false, true>};
   static bool attr_set = false;
   if (!attr_set) {
     for (FwdKernel k : kernels)
@@ -705,7 +696,8 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
         return set_error("cudaFuncSetAttribute(igemm_fwd_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
     attr_set = true;
   }
-  const FwdKernel kernel = kernels[cell ? 3 : A.bn_tile == 32 ? 0 : A.bn_tile == 64 ? 1 : 2];
+  const bool elu = act == VP_ACT_ELU || (aux_y && aux_act == VP_ACT_ELU);
+  const FwdKernel kernel = kernels[cell ? 3 : (A.bn_tile == 32 ? 0 : A.bn_tile == 64 ? 1 : 2) + (elu ? 4 : 0)];
   // persistent over the pixel tiles: one CTA per SM in total; each CTA strides through the M tiles
   const int m_tiles = A.tiles_w * A.tiles_h * A.tiles_d * A.tiles_n;
   const int other = n_tiles * A.num_phases * A.splits;

@@ -5,6 +5,8 @@
 //   PLAIN      Keff = w
 //   POOLED     conv_pool2d (ops.py:838-842): the 2x2 average pool is applied to the kernel
 //   UPSAMPLED  upsample_conv2d (ops.py:698-704): bilinear 4x4 (x) kernel, FULL correlation
+//   DECONV     deconv2d (ops.py:553-590): w is [kh][kw][co][ci], conv2d_transpose's filter layout; Keff = w with the
+//              channel axes swapped
 // and stored K-major, zero padded and rounded to TF32 (round-to-nearest), in the layout the wgmma
 // descriptors read:  FWD  [tap][co -> n_pad][ci -> kc*32],  DGRAD [tap][ci -> n_pad][co -> kc*32].
 // A ConvLSTM's forward packs may interleave the four gates (VP_WLAYOUT_GATES) so that the engine's epilogue holds every
@@ -28,6 +30,8 @@ __device__ __forceinline__ float keff(const float* __restrict__ w, int kind, int
                                       int co_n, int tap, int ci, int co) {
   if (kind == VP_WKIND_PLAIN) {
     return w[(static_cast<long long>(tap) * ci_ref + ci) * co_n + co];
+  } else if (kind == VP_WKIND_DECONV) {
+    return w[(static_cast<long long>(tap) * co_n + co) * ci_ref + ci];
   } else if (kind == VP_WKIND_POOLED) {
     const int P = kw + 1;
     const int p = tap / P, q = tap % P;
@@ -135,7 +139,7 @@ __global__ void unpack_wgrad_kernel(const float* __restrict__ dwp, int kd, int k
   if (cr < 0) return;
   auto at = [&](int tap) { return dwp[(static_cast<long long>(tap) * n_pad + co) * kpad + ci]; };
   float g = 0.f;
-  if (kind == VP_WKIND_PLAIN) {
+  if (kind == VP_WKIND_PLAIN || kind == VP_WKIND_DECONV) {
     g = at(rt);
   } else if (kind == VP_WKIND_POOLED) {
     const int i = rt / kw, j = rt % kw, P = kw + 1;
@@ -148,7 +152,8 @@ __global__ void unpack_wgrad_kernel(const float* __restrict__ dwp, int kd, int k
         if (bw != 0.f) g += bw * at(p * P + q);
       }
   }
-  dw[(static_cast<long long>(rt) * ci_ref + cr) * co_n + co] += g;
+  if (kind == VP_WKIND_DECONV) dw[(static_cast<long long>(rt) * co_n + co) * ci_ref + cr] += g;
+  else dw[(static_cast<long long>(rt) * ci_ref + cr) * co_n + co] += g;
 }
 
 }  // namespace vp
@@ -165,7 +170,8 @@ extern "C" int vp_pack_weights(const float* w, int kd, int kh, int kw, int ci_re
                                const int32_t* cmap, int ci_int, const float* inv_scale, float* wpacked, int n_pad,
                                int kc, vp_stream_t stream) {
   if (!w || !wpacked) return set_error("vp_pack_weights: null pointer");
-  if (kind != VP_WKIND_PLAIN && kd != 1) return set_error("vp_pack_weights: pooled/upsampled kernels are 2-D");
+  if (kind < VP_WKIND_PLAIN || kind > VP_WKIND_DECONV) return set_error("vp_pack_weights: unknown kind %d", kind);
+  if ((kind == VP_WKIND_POOLED || kind == VP_WKIND_UPSAMPLED) && kd != 1) return set_error("vp_pack_weights: pooled/upsampled kernels are 2-D");
   const int taps = eff_taps(kd, kh, kw, kind);
   const int kpad = kc * 32;
   const int rows = (layout & 3) == VP_WLAYOUT_FWD ? co : ci_int, cols = (layout & 3) == VP_WLAYOUT_FWD ? ci_int : co;
@@ -187,6 +193,7 @@ extern "C" int vp_pack_weights_batch(const vp_pack_job* jobs_device, int njobs, 
 extern "C" int vp_unpack_wgrad(const float* dwpacked, int kd, int kh, int kw, int ci_ref, int co, int kind,
                                const int32_t* cmap, int ci_int, float* dw, int n_pad, int kc, vp_stream_t stream) {
   if (!dwpacked || !dw) return set_error("vp_unpack_wgrad: null pointer");
+  if (kind < VP_WKIND_PLAIN || kind > VP_WKIND_DECONV) return set_error("vp_unpack_wgrad: unknown kind %d", kind);
   const long long total = static_cast<long long>(kd) * kh * kw * ci_int * co;
   unpack_wgrad_kernel<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(dwpacked, kd, kh, kw, ci_ref, co, kind, cmap,
                                                                          ci_int, dw, n_pad, kc * 32);

@@ -20,6 +20,7 @@
 #include <mutex>
 #include <tuple>
 
+#include "act.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -28,22 +29,6 @@ namespace cg = cooperative_groups;
 namespace vp {
 
 __device__ __forceinline__ float p_sigm(float v) { return 1.f / (1.f + __expf(-v)); }
-__device__ __forceinline__ float p_act(float v, int act, float alpha) {
-  switch (act) {
-    case VP_ACT_RELU: return fmaxf(v, 0.f);
-    case VP_ACT_LRELU: return fmaxf(alpha * v, v);
-    case VP_ACT_SIGMOID: return p_sigm(v);
-    case VP_ACT_TANH: return tanhf(v);
-    default: return v;
-  }
-}
-__device__ __forceinline__ float p_act_grad(float yp, int act, float alpha) {
-  switch (act) {
-    case VP_ACT_RELU: return yp > 0.f ? 1.f : 0.f;
-    case VP_ACT_LRELU: return yp > 0.f ? 1.f : alpha;
-    default: return 1.f;
-  }
-}
 
 constexpr int kSlabMaxWarps = 16;
 
@@ -98,7 +83,7 @@ struct SlabDsts {
 
 // ------------------------------------------------------------------------------------------------ instance norm forward
 // grid (cluster rank = position slice, slab, sample); block = 8 * lanes; every thread owns ITERS positions x 4 channels.
-template <int ITERS>
+template <int ITERS, bool kElu>
 __global__ void __launch_bounds__(512) slab_inorm_act_kernel(const float* __restrict__ x, int xs, float* __restrict__ y, int ys, int P, int C,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                                              int act, float alpha, float* __restrict__ stats, int cs) {
@@ -137,8 +122,8 @@ __global__ void __launch_bounds__(512) slab_inorm_act_kernel(const float* __rest
 #pragma unroll
   for (int it = 0; it < ITERS; ++it) {
     float4 o;
-    o.x = p_act(v[it].x * g[0] + b[0], act, alpha); o.y = p_act(v[it].y * g[1] + b[1], act, alpha);
-    o.z = p_act(v[it].z * g[2] + b[2], act, alpha); o.w = p_act(v[it].w * g[3] + b[3], act, alpha);
+    o.x = act_fwd<kElu>(v[it].x * g[0] + b[0], act, alpha); o.y = act_fwd<kElu>(v[it].y * g[1] + b[1], act, alpha);
+    o.z = act_fwd<kElu>(v[it].z * g[2] + b[2], act, alpha); o.w = act_fwd<kElu>(v[it].w * g[3] + b[3], act, alpha);
     *reinterpret_cast<float4*>(yp + static_cast<long long>(p0 + pl + it * lanes) * ys) = o;
   }
   if (cs > 1) cg::this_cluster().sync();      // keep this CTA's shared memory alive until every peer has read its partials
@@ -146,7 +131,7 @@ __global__ void __launch_bounds__(512) slab_inorm_act_kernel(const float* __rest
 
 // ------------------------------------------------------------------------------------------------ instance norm backward
 // dx = r*g*(dyp - mean(dyp) - xh*mean(dyp*xh)),  dyp = dy*act'(g*xh+b); dgamma += sum dyp*xh, dbeta += sum dyp
-template <int ITERS>
+template <int ITERS, bool kElu>
 __global__ void __launch_bounds__(512) slab_inorm_act_bwd_kernel(const float* __restrict__ x, int xs, SlabSrcs srcs, float* __restrict__ dx,
                                                                  int dxs, int P, int C, const float* __restrict__ gamma,
                                                                  const float* __restrict__ beta, const float* __restrict__ stats, int act,
@@ -180,7 +165,7 @@ __global__ void __launch_bounds__(512) slab_inorm_act_bwd_kernel(const float* __
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       xh[it][i] = (xv4[i] - m[i]) * r[i];
-      dyp[it][i] = dv[i] * p_act_grad(g[i] * xh[it][i] + b[i], act, alpha);
+      dyp[it][i] = dv[i] * act_grad_pre<kElu>(g[i] * xh[it][i] + b[i], act, alpha);
       s[i] += dyp[it][i];
       s[4 + i] += dyp[it][i] * xh[it][i];
     }
@@ -207,6 +192,7 @@ __global__ void __launch_bounds__(512) slab_inorm_act_bwd_kernel(const float* __
 
 // The same for CTAs that walk more positions than fit in registers (64x64 planes in clusters of 4 = 1024 positions per CTA, so
 // that all 128 CTAs of a 32-sample launch are resident at once): two passes over x and dy, the second one served by the L2.
+template <bool kElu>
 __global__ void __launch_bounds__(512) slab_inorm_act_bwd_loop_kernel(const float* __restrict__ x, int xs, SlabSrcs srcs, float* __restrict__ dx,
                                                                       int dxs, int P, int C, const float* __restrict__ gamma,
                                                                       const float* __restrict__ beta, const float* __restrict__ stats, int act,
@@ -236,7 +222,7 @@ __global__ void __launch_bounds__(512) slab_inorm_act_bwd_loop_kernel(const floa
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       xh[i] = (xv4[i] - m[i]) * r[i];
-      dyp[i] = dv[i] * p_act_grad(g[i] * xh[i] + b[i], act, alpha);
+      dyp[i] = dv[i] * act_grad_pre<kElu>(g[i] * xh[i] + b[i], act, alpha);
     }
   };
   float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -650,13 +636,14 @@ int slab_inorm_act(const float* x, int xs, float* y, int ys, int n, int P, int C
                    float alpha, float* stats, vp_stream_t stream) {
   if (!slab_enabled() || C % 32 || (xs & 3) || (ys & 3)) return 1;
   typedef void (*K)(const float*, int, float*, int, int, int, const float*, const float*, float, int, float, float*, int);
-  auto pick = [](int iters) -> K {
+  const bool elu = act == VP_ACT_ELU;
+  auto pick = [elu](int iters) -> K {
     switch (iters) {
-      case 1: return slab_inorm_act_kernel<1>;
-      case 2: return slab_inorm_act_kernel<2>;
-      case 4: return slab_inorm_act_kernel<4>;
-      case 8: return slab_inorm_act_kernel<8>;
-      case 16: return slab_inorm_act_kernel<16>;
+      case 1: return elu ? slab_inorm_act_kernel<1, true> : slab_inorm_act_kernel<1, false>;
+      case 2: return elu ? slab_inorm_act_kernel<2, true> : slab_inorm_act_kernel<2, false>;
+      case 4: return elu ? slab_inorm_act_kernel<4, true> : slab_inorm_act_kernel<4, false>;
+      case 8: return elu ? slab_inorm_act_kernel<8, true> : slab_inorm_act_kernel<8, false>;
+      case 16: return elu ? slab_inorm_act_kernel<16, true> : slab_inorm_act_kernel<16, false>;
       default: return nullptr;
     }
   };
@@ -677,15 +664,17 @@ int slab_inorm_act_bwd(const float* x, int xs, const float* const* dy, const int
                        vp_stream_t stream) {
   if (!slab_enabled() || C % 32 || (xs & 3) || (dxs & 3)) return 1;
   typedef void (*K)(const float*, int, SlabSrcs, float*, int, int, int, const float*, const float*, const float*, int, float, float*, float*, int);
-  auto pick = [](int iters) -> K {
+  const bool elu = act == VP_ACT_ELU;
+  auto pick = [elu](int iters) -> K {
     switch (iters) {
-      case 1: return slab_inorm_act_bwd_kernel<1>;
-      case 2: return slab_inorm_act_bwd_kernel<2>;
-      case 4: return slab_inorm_act_bwd_kernel<4>;
-      case 8: return slab_inorm_act_bwd_kernel<8>;
+      case 1: return elu ? slab_inorm_act_bwd_kernel<1, true> : slab_inorm_act_bwd_kernel<1, false>;
+      case 2: return elu ? slab_inorm_act_bwd_kernel<2, true> : slab_inorm_act_bwd_kernel<2, false>;
+      case 4: return elu ? slab_inorm_act_bwd_kernel<4, true> : slab_inorm_act_bwd_kernel<4, false>;
+      case 8: return elu ? slab_inorm_act_bwd_kernel<8, true> : slab_inorm_act_bwd_kernel<8, false>;
       default: return nullptr;
     }
   };
+  const auto loop = elu ? slab_inorm_act_bwd_loop_kernel<true> : slab_inorm_act_bwd_loop_kernel<false>;
   // dx may alias one of the gradient sources only in the register-resident kernels (everything is read before anything is written)
   bool aliased = false;
   for (int i = 0; i < num_dy; ++i) aliased = aliased || dy[i] == dx;
@@ -695,7 +684,7 @@ int slab_inorm_act_bwd(const float* x, int xs, const float* const* dy, const int
                    K kk = pick(iters);
                    *threads = lanes * 8; *smem = 0;
                    if (kk) { *kern = reinterpret_cast<const void*>(kk); return true; }
-                   *kern = reinterpret_cast<const void*>(slab_inorm_act_bwd_loop_kernel);
+                   *kern = reinterpret_cast<const void*>(loop);
                    return !aliased && ppc <= 2048;
                  }, &pl)) return 1;
   SlabSrcs s;
@@ -709,7 +698,7 @@ int slab_inorm_act_bwd(const float* x, int xs, const float* const* dy, const int
   float *wg = ws, *wb = ws + static_cast<long long>(n) * C;
   int rc;
   if (!k)
-    rc = launch_cluster(slab_inorm_act_bwd_loop_kernel, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta,
+    rc = launch_cluster(loop, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta,
                         stats, act, alpha, wg, wb, pl.cs, pl.ppc);
   else
     rc = launch_cluster(k, grid, pl.lanes * 8, 0, pl.cs, as_stream(stream), x, xs, s, dx, dxs, P, C, gamma, beta, stats, act, alpha, wg, wb,
@@ -855,6 +844,7 @@ __device__ __forceinline__ void ln_reduce2(float& a, float& b, float* s_warp, fl
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 // grid = n clusters of cs CTAs along x.  stats [n][2] = (mean, rstd).
+template <bool kElu>
 __global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_kernel(const float* __restrict__ x, int xs, float* __restrict__ y, int ys, int P,
                                                                   int C, const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                   float eps, int act, float alpha, float* __restrict__ stats, int lanes,
@@ -894,8 +884,8 @@ __global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_kernel(const float* _
     for (int p = p0 + l; p < p1; p += lanes) {
       const float4 v = ld4(xp + static_cast<long long>(p) * xs);
       float4 o;
-      o.x = p_act(v.x * g[0] + bb[0], act, alpha); o.y = p_act(v.y * g[1] + bb[1], act, alpha);
-      o.z = p_act(v.z * g[2] + bb[2], act, alpha); o.w = p_act(v.w * g[3] + bb[3], act, alpha);
+      o.x = act_fwd<kElu>(v.x * g[0] + bb[0], act, alpha); o.y = act_fwd<kElu>(v.y * g[1] + bb[1], act, alpha);
+      o.z = act_fwd<kElu>(v.z * g[2] + bb[2], act, alpha); o.w = act_fwd<kElu>(v.w * g[3] + bb[3], act, alpha);
       *reinterpret_cast<float4*>(yp + static_cast<long long>(p) * ys) = o;
     }
   }
@@ -906,6 +896,7 @@ __global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_kernel(const float* _
 // The per-channel sums of dyp * xh and dyp: lanes in order within a CTA, then rank 0 adds the CTAs' rows in rank order
 // through DSMEM into row n of wg / wb.  dx may alias x or a dy source: every element is read and written by the same
 // thread, and read before it is written.
+template <bool kElu>
 __global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_bwd_kernel(const float* __restrict__ x, int xs, SlabSrcs srcs, float* dx, int dxs,
                                                                       int P, int C, const float* __restrict__ gamma,
                                                                       const float* __restrict__ beta, const float* __restrict__ stats,
@@ -939,7 +930,7 @@ __global__ void __launch_bounds__(kLnMaxThreads) lnorm_act_bwd_kernel(const floa
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       xh[i] = (xv4[i] - m) * r;
-      dyp[i] = dv[i] * p_act_grad(g[i] * xh[i] + be[i], act, alpha);
+      dyp[i] = dv[i] * act_grad_pre<kElu>(g[i] * xh[i] + be[i], act, alpha);
     }
   };
   float a = 0.f, b = 0.f;
@@ -1017,9 +1008,10 @@ extern "C" int vp_lnorm_act(const float* x, int x_cstride, float* y, int y_cstri
   if (n < 1 || positions < 1 || c < 4) return set_error("vp_lnorm_act: empty shape (n %d, positions %d, c %d)", n, positions, c);
   if (c % 4 || x_cstride % 4 || y_cstride % 4 || x_cstride < c || y_cstride < c)
     return set_error("vp_lnorm_act: channels/strides must be multiples of 4, strides >= channels");
+  if (check_act(act, "vp_lnorm_act")) return -1;
   LnPlan pl;
   if (!plan_lnorm(positions, c, &pl)) return set_error("vp_lnorm_act: at most %d channels", 4 * kLnMaxThreads);
-  return launch_cluster(lnorm_act_kernel, dim3(pl.cs * n), pl.threads, 0, pl.cs, as_stream(stream), x, x_cstride, y, y_cstride, positions,
+  return launch_cluster(act == VP_ACT_ELU ? lnorm_act_kernel<true> : lnorm_act_kernel<false>, dim3(pl.cs * n), pl.threads, 0, pl.cs, as_stream(stream), x, x_cstride, y, y_cstride, positions,
                         c, gamma, beta, eps, act, alpha, stats, pl.lanes, pl.ppc, pl.cs);
 }
 
@@ -1032,6 +1024,7 @@ extern "C" int vp_lnorm_act_bwd(const float* x, int x_cstride, const float* cons
   bool ok = c % 4 == 0 && x_cstride % 4 == 0 && dx_cstride % 4 == 0 && x_cstride >= c && dx_cstride >= c;
   for (int i = 0; i < num_dy; ++i) ok = ok && dy[i] && dy_cstride[i] % 4 == 0 && dy_cstride[i] >= c;
   if (!ok) return set_error("vp_lnorm_act_bwd: null source, or channels/strides not multiples of 4 / strides below channels");
+  if (check_act(act, "vp_lnorm_act_bwd")) return -1;
   LnPlan pl;
   if (!plan_lnorm(positions, c, &pl)) return set_error("vp_lnorm_act_bwd: at most %d channels", 4 * kLnMaxThreads);
   SlabSrcs s;
@@ -1041,7 +1034,7 @@ extern "C" int vp_lnorm_act_bwd(const float* x, int x_cstride, const float* cons
   float* ws = nullptr;
   if (scratch_alloc(&ws, 2LL * n * c, stream)) return -1;
   float *wg = ws, *wb = ws + static_cast<long long>(n) * c;
-  int rc = launch_cluster(lnorm_act_bwd_kernel, dim3(n * pl.cs), pl.threads, static_cast<size_t>(pl.threads) * 8 * sizeof(float), pl.cs,
+  int rc = launch_cluster(act == VP_ACT_ELU ? lnorm_act_bwd_kernel<true> : lnorm_act_bwd_kernel<false>, dim3(n * pl.cs), pl.threads, static_cast<size_t>(pl.threads) * 8 * sizeof(float), pl.cs,
                           as_stream(stream), x, x_cstride, s, dx, dx_cstride, positions, c, gamma, beta, stats, act, alpha, wg, wb,
                           pl.lanes, pl.ppc, pl.cs);
   if (rc == 0) rc = reduce_parts(wg, n, c, dgamma, stream);

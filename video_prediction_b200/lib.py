@@ -26,8 +26,8 @@ class VpConvGeom(C.Structure):
                 ('transposed', C.c_int32)]
 
 
-ACT_NONE, ACT_RELU, ACT_LRELU, ACT_SIGMOID, ACT_TANH = range(5)
-WKIND_PLAIN, WKIND_POOLED, WKIND_UPSAMPLED = range(3)
+ACT_NONE, ACT_RELU, ACT_LRELU, ACT_SIGMOID, ACT_TANH, ACT_ELU = range(6)
+WKIND_PLAIN, WKIND_POOLED, WKIND_UPSAMPLED, WKIND_DECONV = range(4)
 WLAYOUT_FWD, WLAYOUT_DGRAD = range(2)
 WLAYOUT_RESIDUAL = 4
 WLAYOUT_GATES = 8        # OR-ed into a forward layout: the gate-interleaved pack of a ConvLSTM (vp_conv_lstm_fwd)
@@ -258,6 +258,8 @@ class PackPlan(object):
         blocks = 0
         self.keep = entries                                   # the table holds raw pointers: keep the tensors alive
         for j, (w, k, ci_ref, co, kind, layout, ci_int, cmap, inv_scale, out) in zip(jobs, entries):
+            if kind not in (WKIND_PLAIN, WKIND_POOLED, WKIND_UPSAMPLED, WKIND_DECONV):
+                raise VpError('PackPlan: unknown weight kind %r' % (kind,))     # vp_pack_weights rejects it the same way
             ci_int = ci_ref if ci_int is None else ci_int
             n_pad, kc, total = pack_dims(k, ci_int, co, kind, layout)
             assert out.numel() == total and w.is_contiguous()

@@ -182,6 +182,30 @@ def conv3x(x, c, geom, wp, wp_lo, n_pad, kc, ov, bias, act, alpha, accumulate=Fa
         L.conv_igemm_actgrad(xv, geom, wp_lo, n_pad, kc, ov, aux[0], aux[1], aux[2], alpha, accumulate=2)
 
 
+# The generator's h{i} convolutions (savp_model.py:394-397, 461-464, 494-500; ops.get_downsample_layer /
+# get_upsample_layer, ops.py:1077-1098): name -> (variable scope, weight kind, pad before, transposed), all with stride 2.
+# The kernel is [k, k, cin, oc] -- deconv2d's is [3, 3, oc, cin], conv2d_transpose's filter layout.
+#   conv_pool2d:  SAME conv + 2x2 average pool, folded into one (k+1)x(k+1) stride-2 conv (pad before k // 2)
+#   conv2d:       k x k stride-2 SAME conv; SAME on an even extent pads (k-2) // 2 before, the rest after
+#   upsample_conv2d: bilinear 2x upsample + 3x3 conv, folded into one 6x6 transposed conv (pad 2)
+#   deconv2d:     3x3 stride-2 conv2d_transpose, the adjoint of the 2H -> H SAME conv (pad 0 before, 1 after)
+# The _v2 recipes compute the same functions as the v1 layers with the v1 variables (ops.py:643-680, 795-820), so they
+# run on the v1 packs.
+DOWNSAMPLE_LAYERS = {
+    'conv_pool2d': ('conv_pool2d', L.WKIND_POOLED, lambda k: k // 2, False),
+    'conv_pool2d_v2': ('conv_pool2d', L.WKIND_POOLED, lambda k: k // 2, False),
+    'conv2d': ('conv2d', L.WKIND_PLAIN, lambda k: (k - 2) // 2, False),
+}
+UPSAMPLE_LAYERS = {
+    'upsample_conv2d': ('upsample_conv2d', L.WKIND_UPSAMPLED, lambda k: 2, True),
+    'upsample_conv2d_v2': ('upsample_conv2d', L.WKIND_UPSAMPLED, lambda k: 2, True),
+    'deconv2d': ('deconv2d', L.WKIND_DECONV, lambda k: 0, True),
+}
+# activation_layer (ops.get_activation_layer, ops.py:1052-1059): the activation of every norm_layer site of the generator
+# (h{i} and the h_flow / h_scratch / h_masks heads); the posterior encoder keeps its leaky relu
+ACTIVATIONS = {'relu': L.ACT_RELU, 'elu': L.ACT_ELU}
+
+
 class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
     def __init__(self, *args, **kwargs):
         super(SAVPVideoPredictionModel, self).__init__(*args, **kwargs)
@@ -234,10 +258,12 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise NotImplementedError('schedule_sampling=%r' % (hp.schedule_sampling,))     # savp_model.py:332-333
         if hp.gan_loss_type not in ('LSGAN', 'GAN', 'SNGAN'):
             raise ValueError('Unknown GAN loss type %s' % hp.gan_loss_type)                 # losses.py:52-53
+        for key, table in (('downsample', DOWNSAMPLE_LAYERS), ('upsample', UPSAMPLE_LAYERS), ('activation', ACTIVATIONS)):
+            if getattr(hp, key + '_layer') not in table:      # ops.get_*_layer (ops.py:1052-1098)
+                raise ValueError('Invalid %s layer %s' % (key, getattr(hp, key + '_layer')))
         unsupported = []
         for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('downsample_layer', 'conv_pool2d'),
-                          ('upsample_layer', 'upsample_conv2d'), ('activation_layer', 'relu'), ('last_frames', 1),
+                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('last_frames', 1),
                           ('prev_image_background', True), ('first_image_background', True),
                           ('last_image_background', False), ('last_context_image_background', False),
                           ('context_images_background', False), ('generate_scratch_image', True),
@@ -287,6 +313,24 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         layers 2..): the default scope of the layer ops.get_norm_layer picks (ops.py:1062-1073), or None for
         norm_layer='none' (tf.identity, no variables).  The ConvLSTM's own norms follow conv_rnn_norm_layer instead."""
         return {'instance': 'InstanceNorm', 'layer': 'LayerNorm'}.get(self.hparams.norm_layer)
+
+    @property
+    def site_act(self):
+        """The activation of the generator's norm_layer sites (activation_layer)."""
+        return ACTIVATIONS[self.hparams.activation_layer]
+
+    def _hconv_layer(self, li, cin, oc):
+        """(scope, kernel shape, weight kind, kernel size, pad before, transposed) of the h{li} convolution with cin input
+        channels (tile-concat included)."""
+        hp = self.hparams
+        if li < len(self.enc_specs):
+            ks = 5 if li == 0 else 3
+            scope, kind, pad, transposed = DOWNSAMPLE_LAYERS[hp.downsample_layer]
+        else:
+            ks = 3
+            scope, kind, pad, transposed = UPSAMPLE_LAYERS[hp.upsample_layer]
+        shape = (ks, ks, oc, cin) if kind == L.WKIND_DECONV else (ks, ks, cin, oc)
+        return '%s/h%d/%s' % ('generator/rnn/savp_cell', li, scope), shape, kind, ks, pad(ks), transposed
 
     # ------------------------------------------------------------------ structure (savp_model.py:182-232)
     @staticmethod
@@ -356,9 +400,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         outs = []
         cin = 2 * C
         for i, (oc, use) in enumerate(enc):
-            ks = 5 if i == 0 else 3
-            specs['%s/h%d/conv_pool2d/kernel' % (sc, i)] = ((ks, ks, cin + Zc, oc), 'kernel')
-            specs['%s/h%d/conv_pool2d/bias' % (sc, i)] = ((oc,), 'zeros')
+            scope, shape = self._hconv_layer(i, cin + Zc, oc)[:2]
+            specs[scope + '/kernel'] = (shape, 'kernel')
+            specs[scope + '/bias'] = ((oc,), 'zeros')
             site_norm('%s/h%d' % (sc, i), oc)
             if use:
                 lstm(i, oc, oc)
@@ -368,8 +412,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         for i, (oc, use) in enumerate(dec):
             li = n_enc + i
             cin = outs[-1] if i == 0 else outs[-1] + outs[n_enc - i - 1]
-            specs['%s/h%d/upsample_conv2d/kernel' % (sc, li)] = ((3, 3, cin + Zc, oc), 'kernel')
-            specs['%s/h%d/upsample_conv2d/bias' % (sc, li)] = ((oc,), 'zeros')
+            scope, shape = self._hconv_layer(li, cin + Zc, oc)[:2]
+            specs[scope + '/kernel'] = (shape, 'kernel')
+            specs[scope + '/bias'] = ((oc,), 'zeros')
             site_norm('%s/h%d' % (sc, li), oc)
             if use:
                 lstm(li, oc, oc)
@@ -766,15 +811,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 segs = [('x', outs[-1]), ('skip', outs[n_enc - (li - n_enc) - 1])] + zseg
             d['in_spec'] = ConcatSpec(segs)
             Bf['in%d' % li] = self._z(S, NB, ih, iw, d['in_spec'].cstride)
-            if is_enc:
-                ks = 5 if li == 0 else 3
-                pb = (ks + 1 - 2) // 2
-                d['conv'] = ConvLayer(self, '%s/h%d/conv_pool2d/kernel' % (sc, li), '%s/h%d/conv_pool2d/bias' % (sc, li),
-                                      (1, ks, ks), L.WKIND_POOLED, (1, 2, 2), (0, pb, pb), False, d['in_spec'], oc)
-            else:
-                d['conv'] = ConvLayer(self, '%s/h%d/upsample_conv2d/kernel' % (sc, li),
-                                      '%s/h%d/upsample_conv2d/bias' % (sc, li), (1, 3, 3), L.WKIND_UPSAMPLED, (1, 2, 2),
-                                      (0, 2, 2), True, d['in_spec'], oc)
+            scope, _, kind, ks, pb, transposed = self._hconv_layer(li, d['in_spec'].ref_channels, oc)
+            d['conv'] = ConvLayer(self, scope + '/kernel', scope + '/bias', (1, ks, ks), kind, (1, 2, 2), (0, pb, pb), transposed,
+                                  d['in_spec'], oc)
             self.convs.append(d['conv'])
             Bf['pre%d' % li] = self._z(S, NB, hh, ww, oc)
             Bf['nst%d' % li] = self._norm_stats(S, NB, oc)
@@ -1188,8 +1227,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             if d['use']:
                 rsp = d['rin_spec']
                 rin = Bf['rin%d' % li][t]
-                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, rin, rsp.off('x'))
-                self._site_norm(site, pre, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc, L.ACT_RELU, 0.0,
+                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, rin, rsp.off('x'), act=self.site_act)
+                self._site_norm(site, pre, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc, self.site_act, 0.0,
                                 Bf['nst%d' % li][t])
                 gpre = Bf['gpre%d' % li][t]
                 b = d['rname']
@@ -1213,8 +1252,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             else:
                 dests = self._h_dests(li, t)
                 out = Bf['out%d' % li][t]
-                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, out)
-                self._site_norm(site, pre, out.data_ptr(), oc, NB, hh * ww, oc, L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
+                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, out, act=self.site_act)
+                self._site_norm(site, pre, out.data_ptr(), oc, NB, hh * ww, oc, self.site_act, 0.0, Bf['nst%d' % li][t])
                 for addr, cs in dests:
                     L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
         nk, kh, kw = self.nk, self.kh, self.kw
@@ -1223,8 +1262,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         nl = self.nl
         if self.flow:
             # flow heads (savp_model.py:522-530): h_flow = relu(IN(conv3x3(top))), flows = conv3x3(h_flow) [.., 2, nk]
-            self._site_conv(self.conv_hflow, top, Bf['fpre'][t], Bf['hf'][t])
-            self._site_norm('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, L.ACT_RELU, 0.0,
+            self._site_conv(self.conv_hflow, top, Bf['fpre'][t], Bf['hf'][t], act=self.site_act)
+            self._site_norm('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act, 0.0,
                             Bf['fst'][t])
             self.conv_flows.fwd(Bf['hf'][t], Bf['flows'][t], out_c=2 * nk)
         else:
@@ -1238,12 +1277,12 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         # heads
         mk = Bf['mk'][t]
         msp = self.mk_spec
-        self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t])
-        self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'))
-        self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, L.ACT_RELU, 0.0,
+        self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t], act=self.site_act)
+        self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'), act=self.site_act)
+        self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act, 0.0,
                         Bf['sst'][t])
         self._site_norm('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
-                        L.ACT_RELU, 0.0, Bf['mst'][t])
+                        self.site_act, 0.0, Bf['mst'][t])
         # scratch image -> last layer slot (savp_model.py:570-572, 595-596)
         self.conv_simg.fwd(Bf['hs'][t], mk, out_off=msp.off('l%d' % (self.nlayers - 1)), out_c=C, act=L.ACT_SIGMOID)
         # transformed images: 4 CDNA (or flow-warped) + prev image + first image (savp_model.py:574-584)

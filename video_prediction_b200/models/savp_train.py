@@ -337,7 +337,7 @@ class TrainMixin(object):
         self.conv_masks.dgrad(G['dmlog'][t], dmk, dy_c=nlay)
         # h_masks branch
         self._site_norm_bwd('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride,
-                            [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, L.ACT_RELU, 0.0,
+                            [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, self.site_act, 0.0,
                             Bf['mst'][t])
         self.conv_hmasks.dgrad(G['dmpre'][t], G['dtop'][t])
         # scratch branch
@@ -346,7 +346,7 @@ class TrainMixin(object):
                   G['dlay'][t].data_ptr() + 4 * 4 * (nlay - 1), 4 * nlay, G['dsimg'][t].data_ptr(), 4, NB * HW, C, L.ACT_SIGMOID)
         self.conv_simg.dgrad(G['dsimg'][t], G['dhs'][t], dy_c=C)
         self._site_norm_bwd('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, [(G['dhs'][t].data_ptr(), ngf)],
-                            G['dspre'][t], NB, HW, ngf, L.ACT_RELU, 0.0, Bf['sst'][t])
+                            G['dspre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['sst'][t])
         self.conv_scratch.dgrad(G['dspre'][t], G['dtop'][t], accumulate=True)
         nk, kh, kw = self.nk, self.kh, self.kw
         G['dimg'][t].zero_()
@@ -356,7 +356,7 @@ class TrainMixin(object):
                              G['dlay'][t].data_ptr(), 4 * nlay, G['dimg'][t], G['dflows'][t], NB, H, W, nk)
             self.conv_flows.dgrad(G['dflows'][t], G['dhf'][t], dy_c=2 * nk)
             self._site_norm_bwd('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, [(G['dhf'][t].data_ptr(), ngf)],
-                                G['dfpre'][t], NB, HW, ngf, L.ACT_RELU, 0.0, Bf['fst'][t])
+                                G['dfpre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['fst'][t])
             self.conv_hflow.dgrad(G['dfpre'][t], G['dtop'][t], accumulate=True)
         else:
             # CDNA
@@ -418,7 +418,7 @@ class TrainMixin(object):
             else:
                 y_addr, y_cs = Bf['out%d' % li][t].data_ptr(), oc
             self._site_norm_bwd('%s/h%d' % (sc, li), Bf['pre%d' % li][t], y_addr, y_cs, srcs, G['dpre%d' % li][t], NB, hh * ww, oc,
-                                L.ACT_RELU, 0.0, Bf['nst%d' % li][t])
+                                self.site_act, 0.0, Bf['nst%d' % li][t])
             d['conv'].dgrad(G['dpre%d' % li][t], G['din%d' % li][t])
         # gradient w.r.t. the input image of this step: CDNA path + first conv's 'image' slot
         sp = self.gl[0]['in_spec']

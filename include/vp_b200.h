@@ -191,6 +191,34 @@ int vp_cdna_kernel_norm(const float* raw, float* out, int b, int kh, int kw, int
  * layers[(n*h*w+p)*layers_cstride + 4*l]. */
 int vp_cdna_apply(const float* image, const float* first_image, const float* kernels, float* layers,
                   int layers_cstride, int n, int h, int w, int kh, int kw, int nk, vp_stream_t stream);
+/* Slot writer of the compositing stage (savp_model.py:574-596), the general form of vp_cdna_apply: the masks-conv concat
+ * buffer gets, as float4 slots layers[(n*h*w + p)*layers_cstride + 4*l]:
+ *   slot k < nk        = transform k (apply_cdna_kernels, :893-923, SYMMETRIC padding) of frames[k / (nk / nframes)];
+ *                        kernels [n][kh*kw][nk], frames [nframes][n][h][w][4] the history images oldest first (:926-965)
+ *   slot nk + b < nk+nbg = backgrounds[b] [n][h][w][4], copied
+ * Limits: nk <= VP_SLOT_MAX_TRANSFORMS, nk % nframes == 0, nframes <= VP_SLOT_MAX_FRAMES, nk + nbg <= VP_SLOT_MAX_LAYERS.
+ * frames / backgrounds are HOST arrays of device pointers, read at the call (the table is a kernel argument, so a captured
+ * graph keeps the pointers of the capture).  frames may be NULL when nk == 0. */
+#define VP_SLOT_MAX_TRANSFORMS 16
+#define VP_SLOT_MAX_FRAMES 16
+#define VP_SLOT_MAX_LAYERS 32
+int vp_cdna_slots(const float* const* frames, int nframes, const float* kernels, int nk, const float* const* backgrounds,
+                  int nbg, float* layers, int layers_cstride, int n, int h, int w, int kh, int kw, vp_stream_t stream);
+/* The same with transformation='flow': transform k warps frames[k / (nk / nframes)] by flows channels (k, nk + k). */
+int vp_flow_slots(const float* const* frames, int nframes, const float* flows, int flows_cstride, int nk,
+                  const float* const* backgrounds, int nbg, float* layers, int layers_cstride, int n, int h, int w,
+                  vp_stream_t stream);
+/* Backward of the slot writers.  dT_l = d_a[.., 4l] + d_b[.., 4l] (the masks conv and the compositor).  dframes[f] (HOST array
+ * of device pointers; NULL = no gradient for that frame) += the gradient of frame f through its transforms, plus, for the
+ * last frame, dT_prev_slot (prev_slot = the slot holding the previous image as a background, -1 = none).  CDNA: dkernels +=
+ * (fixed-order reduction), dframes gathered (no float atomics: identical inputs give identical bits).  Flow: dflows
+ * overwritten, dframes += atomically.  Distinct frames must have distinct dframes. */
+int vp_cdna_slots_bwd(const float* const* frames, int nframes, const float* kernels, int nk, int prev_slot, const float* d_a,
+                      int d_a_cstride, const float* d_b, int d_b_cstride, float* const* dframes, float* dkernels, int n,
+                      int h, int w, int kh, int kw, vp_stream_t stream);
+int vp_flow_slots_bwd(const float* const* frames, int nframes, const float* flows, int flows_cstride, int nk, int prev_slot,
+                      const float* d_a, int d_a_cstride, const float* d_b, int d_b_cstride, float* const* dframes,
+                      float* dflows, int n, int h, int w, vp_stream_t stream);
 /* flow_ops.image_warp (flow_ops.py:4-79; transformation='flow', savp_model.py:955-965): backward bilinear warp with
  * the neighbour indices clipped to the image; flow [n][h][w][2] = (x, y) displacement.  bwd: dim += (atomic, may be
  * NULL), dflow overwritten (may be NULL). */
@@ -198,7 +226,8 @@ int vp_image_warp_fwd(const float* im, int im_cstride, const float* flow, float*
                       int c, vp_stream_t stream);
 int vp_image_warp_bwd(const float* im, int im_cstride, const float* flow, const float* dout, int dout_cstride, float* dim,
                       int dim_cstride, float* dflow, int n, int h, int w, int c, vp_stream_t stream);
-/* masks = softmax(logits) (savp_model.py:634); gen_image = sum_l layer_l * mask_l (:645-646). */
+/* masks = softmax(logits) (savp_model.py:634); gen_image = sum_l layer_l * mask_l (:645-646); 1 <= num_layers <=
+ * VP_SLOT_MAX_LAYERS, logits / masks strides >= num_layers (masks may be NULL). */
 int vp_composite(const float* logits, int logits_cstride, const float* layers, int layers_cstride, float* masks,
                  int masks_cstride, float* gen_image, long long positions, int num_layers, vp_stream_t stream);
 
@@ -283,6 +312,21 @@ int vp_pix_distrib_fwd(const int32_t* sel, const float* pix_gt, const float* pix
                        const float* masks, int masks_cstride, float* gen, int gen_cstride, float* transformed,
                        int transformed_cstride, int slot_stride, int n, int h, int w, int d, int kh, int kw, int nk,
                        vp_stream_t stream);
+
+/* The general form of vp_pix_distrib_fwd for every compositing layout (savp_model.py:598-621): with p the selected map of
+ * this step (as above), the slots are
+ *   slot k < nk        = CDNA_k or warp_k of history map k / (nk / nframes); map nframes - 1 is p, maps f < nframes - 1 are
+ *                        frames[f] (the selected maps of earlier steps, oldest first; frames may be NULL when nframes == 1)
+ *   slot nk + b        = backgrounds[b] (a ground-truth map), or p where backgrounds[b] is NULL (the previous-image slot)
+ *   slot nk + nbg      = p, when scratch (the scratch-image slot takes the map)
+ * composited with masks (masks_cstride >= slots) and normalised per plane as above.  frames, backgrounds and cur_out share
+ * pix_gt's channel stride; cur_out (may be NULL) receives p, the history map of later steps.  1 <= slots <= VP_SLOT_MAX_LAYERS,
+ * nk <= VP_SLOT_MAX_TRANSFORMS; without transforms kernels and flows are NULL. */
+int vp_pix_slots_fwd(const int32_t* sel, const float* pix_gt, int pix_cstride, const float* gen_prev, const float* const* frames,
+                     int nframes, const float* kernels, const float* flows, int flows_cstride, int nk,
+                     const float* const* backgrounds, int nbg, int scratch, const float* masks, int masks_cstride, float* gen,
+                     int gen_cstride, float* transformed, int transformed_cstride, int slot_stride, float* cur_out, int n, int h,
+                     int w, int d, int kh, int kw, vp_stream_t stream);
 
 /* Robot-state recurrence of the action-conditioned cell (savp_model.py:411-412, 655-658), all s steps of n rows in one
  * launch, forward only (no loss reads the predicted states).  For t < s and row r < n:

@@ -269,13 +269,14 @@ __global__ void __launch_bounds__(512) lstm_gates_bwd_kernel(
 // ------------------------------------------------------------------------------------------------
 // compositing backward: dlogit_l = m_l*(g_l - sum_k m_k g_k), g_l = <dgen, layer_l>; dlayer_l = m_l*dgen
 // ------------------------------------------------------------------------------------------------
+template <int kMaxL>
 __global__ void composite_bwd_kernel(const float4* __restrict__ dgen, const float* __restrict__ masks, int ms,
                                      const float* __restrict__ layers, int ls, float* __restrict__ dlogits, int dls,
                                      float* __restrict__ dlayers, int dlays, long long total, int L) {
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const float4 dg = dgen[idx];
-  float m[8], g[8];
+  float m[kMaxL], g[kMaxL];
   float dot = 0.f;
   for (int l = 0; l < L; ++l) {
     m[l] = masks[idx * ms + l];
@@ -285,7 +286,7 @@ __global__ void composite_bwd_kernel(const float4* __restrict__ dgen, const floa
     *reinterpret_cast<float4*>(dlayers + idx * dlays + 4 * l) = make_float4(m[l] * dg.x, m[l] * dg.y, m[l] * dg.z, m[l] * dg.w);
   }
   for (int l = 0; l < L; ++l) dlogits[idx * dls + l] = m[l] * (g[l] - dot);
-  for (int l = L; l < dls && l < 8; ++l) dlogits[idx * dls + l] = 0.f;
+  for (int l = L; l < dls && l < kMaxL; ++l) dlogits[idx * dls + l] = 0.f;
 }
 
 __device__ __forceinline__ int reflect_i(int i, int n) {
@@ -293,13 +294,15 @@ __device__ __forceinline__ int reflect_i(int i, int n) {
   if (i >= n) i = 2 * n - 1 - i;
   return i;
 }
-// CDNA apply backward.  dT_k = dA[.., 4k] + dB[.., 4k] (two gradient sources: compositor + masks conv).
-//  dimage += scatter_k,tap K[tap][k]*dT_k  (+ dprev slot NK)      dkern[n][tap][k] += <dT_k, img[reflect(.+tap)]>
-__global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __restrict__ image, const float* __restrict__ kern,
+// Backward of cdna_slots_kernel.  dT_k = dA[.., 4k] + dB[.., 4k] (two gradient sources: compositor + masks conv); transform
+// k applies to frame k / G, G = NK / NF.
+//  dkern[n][tap][k] = <dT_k, frame_{k/G}[reflect(.+tap)]>, per-block partials (reduced in a fixed order by the caller)
+template <int kMaxNk>
+__global__ void __launch_bounds__(256) cdna_slots_bwd_kernel(const __grid_constant__ VpSlotTable tab, const float* __restrict__ kern,
                                                              const float* __restrict__ dA, int das,
                                                              const float* __restrict__ dB, int dbs,
-                                                             float* __restrict__ dimage, float* __restrict__ dkern, int N,
-                                                             int H, int W, int KH, int KW, int NK) {
+                                                             float* __restrict__ dkern, int N,
+                                                             int H, int W, int KH, int KW, int NK, int NF) {
   extern __shared__ float sk[];  // [KK*NK] kernels, then [8 warps][KK*NK] dkern partials
   const int n = blockIdx.y;
   const int KK = KH * KW;
@@ -310,13 +313,14 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __res
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   const bool valid = p < H * W;
   const int y = valid ? p / W : 0, x = valid ? p % W : 0;
-  const float4* img = image + static_cast<long long>(n) * H * W;
-  float4 dT[4];
+  const long long row = static_cast<long long>(n) * H * W;
+  const int G = NK / NF;
+  float4 dT[kMaxNk];
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
+  for (int k = 0; k < kMaxNk; ++k) {
     dT[k] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (valid && k < NK) {
-      const long long o = (static_cast<long long>(n) * H * W + p);
+      const long long o = row + p;
       const float4 a = *reinterpret_cast<const float4*>(dA + o * das + 4 * k);
       const float4 b = *reinterpret_cast<const float4*>(dB + o * dbs + 4 * k);
       dT[k] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
@@ -329,13 +333,15 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __res
     for (int j = 0; j < KW; ++j) {
       const int xx = reflect_i(x + j - pw, W);
       const int q = yy * W + xx;
-      const float4 v = valid ? img[q] : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int f = 0; f < NF; ++f) {
+        const float4 v = valid ? reinterpret_cast<const float4*>(tab.ptr[f])[row + q] : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (k < NK) {
-          float d = dT[k].x * v.x + dT[k].y * v.y + dT[k].z * v.z + dT[k].w * v.w;
-          d = wsum(d);
-          if (lane == 0) sdk[warp * KK * NK + (i * KW + j) * NK + k] += d;
+        for (int k = 0; k < kMaxNk; ++k) {
+          if (k < NK && k >= f * G && k < (f + 1) * G) {
+            float d = dT[k].x * v.x + dT[k].y * v.y + dT[k].z * v.z + dT[k].w * v.w;
+            d = wsum(d);
+            if (lane == 0) sdk[warp * KK * NK + (i * KW + j) * NK + k] += d;
+          }
         }
       }
     }
@@ -348,25 +354,28 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_kernel(const float4* __res
     dkern[(static_cast<long long>(blockIdx.x) * N + n) * KK * NK + i] = t;
   }
 }
-// dimage[q] += dT_NK[q] + sum_{taps, k} K[tap][k] * dT_k[p] over the pixels p whose reflected tap lands on q: a gather, so every
-// image gradient is summed in the same order on every run.  reflect_i(v) == q for v = q, -q - 1 and 2n - 1 - q.
-__global__ void __launch_bounds__(256) cdna_apply_bwd_dimage_kernel(const float* __restrict__ kern, const float* __restrict__ dA, int das,
-                                                                    const float* __restrict__ dB, int dbs, float* __restrict__ dimage, int N,
-                                                                    int H, int W, int KH, int KW, int NK) {
-  const int n = blockIdx.y;
+// dframe_f[q] += [f == NF-1] dT_PREV[q] + sum_{taps, k in group f} K[tap][k] * dT_k[p] over the pixels p whose reflected tap
+// lands on q (blockIdx.z = f; frames with a NULL dframe are skipped): a gather, so every image gradient is summed in the same
+// order on every run.  reflect_i(v) == q for v = q, -q - 1 and 2n - 1 - q.
+__global__ void __launch_bounds__(256) cdna_slots_bwd_dimage_kernel(const __grid_constant__ VpSlotTable dtab, const float* __restrict__ kern,
+                                                                    const float* __restrict__ dA, int das, const float* __restrict__ dB,
+                                                                    int dbs, int N, int H, int W, int KH, int KW, int NK, int NF, int PREV) {
+  const int n = blockIdx.y, f = blockIdx.z;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= H * W) return;
+  float* dimage = const_cast<float*>(dtab.ptr[f]);
+  if (q >= H * W || !dimage) return;
   const int qy = q / W, qx = q % W;
   const int ph = (KH - 1) / 2, pw = (KW - 1) / 2;
+  const int G = NK / NF, k0 = f * G, k1 = (f + 1) * G;
   const float* kn = kern + static_cast<long long>(n) * KH * KW * NK;
   const long long base = static_cast<long long>(n) * H * W;
-  float3 acc;
-  {
-    const float4 a = *reinterpret_cast<const float4*>(dA + (base + q) * das + 4 * NK);
-    const float4 b = *reinterpret_cast<const float4*>(dB + (base + q) * dbs + 4 * NK);
+  float3 acc = make_float3(0.f, 0.f, 0.f);
+  if (PREV >= 0 && f == NF - 1) {
+    const float4 a = *reinterpret_cast<const float4*>(dA + (base + q) * das + 4 * PREV);
+    const float4 b = *reinterpret_cast<const float4*>(dB + (base + q) * dbs + 4 * PREV);
     acc = make_float3(a.x + b.x, a.y + b.y, a.z + b.z);
   }
-  for (int i = 0; i < KH; ++i) {
+  for (int i = 0; i < KH && NK; ++i) {
     const int vy[3] = {qy, -qy - 1, 2 * H - 1 - qy};
     for (int cy = 0; cy < 3; ++cy) {
       const int py = vy[cy] - i + ph;
@@ -378,7 +387,7 @@ __global__ void __launch_bounds__(256) cdna_apply_bwd_dimage_kernel(const float*
           if (px < 0 || px >= W) continue;
           const long long o = base + static_cast<long long>(py) * W + px;
           const float* kk = kn + (i * KW + j) * NK;
-          for (int k = 0; k < NK; ++k) {
+          for (int k = k0; k < k1; ++k) {
             const float4 a = *reinterpret_cast<const float4*>(dA + o * das + 4 * k);
             const float4 b = *reinterpret_cast<const float4*>(dB + o * dbs + 4 * k);
             acc.x += kk[k] * (a.x + b.x); acc.y += kk[k] * (a.y + b.y); acc.z += kk[k] * (a.z + b.z);
@@ -945,10 +954,60 @@ extern "C" int vp_lstm_gates_bwd(const float* pre, int n, int positions, int fil
 extern "C" int vp_composite_bwd(const float* dgen, const float* masks, int masks_cstride, const float* layers, int layers_cstride,
                                 float* dlogits, int dlogits_cstride, float* dlayers, int dlayers_cstride, long long positions,
                                 int num_layers, vp_stream_t stream) {
-  composite_bwd_kernel<<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(dgen), masks, masks_cstride, layers, layers_cstride, dlogits, dlogits_cstride, dlayers,
-      dlayers_cstride, positions, num_layers);
+  if (num_layers < 1 || num_layers > VP_SLOT_MAX_LAYERS)
+    return set_error("vp_composite_bwd: 1 .. %d layers, got %d", VP_SLOT_MAX_LAYERS, num_layers);
+  if (!dgen || !masks || !layers || !dlogits || !dlayers) return set_error("vp_composite_bwd: null pointer");
+  if (masks_cstride < num_layers || dlogits_cstride < num_layers || layers_cstride < 4 * num_layers ||
+      dlayers_cstride < 4 * num_layers)
+    return set_error("vp_composite_bwd: strides smaller than the %d layers", num_layers);
+  if (num_layers <= 8)
+    composite_bwd_kernel<8><<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(
+        reinterpret_cast<const float4*>(dgen), masks, masks_cstride, layers, layers_cstride, dlogits, dlogits_cstride, dlayers,
+        dlayers_cstride, positions, num_layers);
+  else
+    composite_bwd_kernel<VP_SLOT_MAX_LAYERS><<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(
+        reinterpret_cast<const float4*>(dgen), masks, masks_cstride, layers, layers_cstride, dlogits, dlogits_cstride, dlayers,
+        dlayers_cstride, positions, num_layers);
   return check_launch("composite_bwd_kernel");
+}
+
+extern "C" int vp_cdna_slots_bwd(const float* const* frames, int nframes, const float* kernels, int nk, int prev_slot, const float* d_a,
+                                 int d_a_cstride, const float* d_b, int d_b_cstride, float* const* dframes, float* dkernels, int n,
+                                 int h, int w, int kh, int kw, vp_stream_t stream) {
+  VpSlotTable tab, dtab{};
+  if (slot_table(&tab, frames, nframes, nk, nullptr, 0, "vp_cdna_slots_bwd")) return -1;
+  if (nframes < 1 || nframes > VP_SLOT_MAX_FRAMES || !dframes) return set_error("vp_cdna_slots_bwd: bad frames / dframes");
+  if (!d_a || !d_b || (nk && (!kernels || !dkernels))) return set_error("vp_cdna_slots_bwd: null pointer");
+  if (prev_slot >= VP_SLOT_MAX_LAYERS || prev_slot < -1 || (prev_slot >= 0 && prev_slot < nk))
+    return set_error("vp_cdna_slots_bwd: bad prev_slot %d", prev_slot);
+  if (d_a_cstride % 4 || d_b_cstride % 4) return set_error("vp_cdna_slots_bwd: gradient strides must be multiples of 4");
+  if (n < 1 || h < 1 || w < 1 || n > 65535 || (nk && (kh < 1 || kw < 1)))
+    return set_error("vp_cdna_slots_bwd: bad n / h / w / kernel");
+  if (nk && ((kh - 1) / 2 >= h || (kw - 1) / 2 >= w)) return set_error("vp_cdna_slots_bwd: kernel larger than the image");
+  for (int f = 0; f < nframes; ++f) dtab.ptr[f] = dframes[f];
+  const int nf = nk ? nframes : 1;
+  dim3 grid((h * w + 255) / 256, n);
+  if (nk) {
+    const long long part = static_cast<long long>(n) * kh * kw * nk;
+    float* ws = nullptr;
+    if (scratch_alloc(&ws, grid.x * part, stream)) return -1;
+    const size_t smem = 9 * static_cast<size_t>(kh) * kw * nk * sizeof(float);
+    if (nk <= 4)
+      cdna_slots_bwd_kernel<4><<<grid, 256, smem, as_stream(stream)>>>(tab, kernels, d_a, d_a_cstride, d_b, d_b_cstride, ws, n, h, w, kh,
+                                                                       kw, nk, nf);
+    else
+      cdna_slots_bwd_kernel<VP_SLOT_MAX_TRANSFORMS><<<grid, 256, smem, as_stream(stream)>>>(tab, kernels, d_a, d_a_cstride, d_b, d_b_cstride,
+                                                                                            ws, n, h, w, kh, kw, nk, nf);
+    int rc = check_launch("cdna_slots_bwd_kernel");
+    if (!rc) rc = reduce_parts(ws, grid.x, part, dkernels, stream);
+    scratch_free(ws, stream);
+    if (rc) return rc;
+  }
+  if (!nk && prev_slot < 0) return 0;
+  grid.z = nf;
+  cdna_slots_bwd_dimage_kernel<<<grid, 256, 0, as_stream(stream)>>>(dtab, kernels, d_a, d_a_cstride, d_b, d_b_cstride, n, h, w, kh, kw,
+                                                                    nk, nf, prev_slot);
+  return check_launch("cdna_slots_bwd_dimage_kernel");
 }
 
 extern "C" int vp_cdna_apply_bwd(const float* image, const float* kernels, const float* d_a, int d_a_cstride, const float* d_b,
@@ -956,18 +1015,7 @@ extern "C" int vp_cdna_apply_bwd(const float* image, const float* kernels, const
                                  vp_stream_t stream) {
   if (nk > 4) return set_error("vp_cdna_apply_bwd: at most 4 transformations");
   if ((kh - 1) / 2 >= h || (kw - 1) / 2 >= w) return set_error("vp_cdna_apply_bwd: kernel larger than the image");
-  dim3 grid((h * w + 255) / 256, n);
-  const long long part = static_cast<long long>(n) * kh * kw * nk;
-  float* ws = nullptr;
-  if (scratch_alloc(&ws, grid.x * part, stream)) return -1;
-  cdna_apply_bwd_kernel<<<grid, 256, 9 * kh * kw * nk * sizeof(float), as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(image), kernels, d_a, d_a_cstride, d_b, d_b_cstride, dimage, ws, n, h, w, kh, kw, nk);
-  int rc = check_launch("cdna_apply_bwd_kernel");
-  if (!rc) rc = reduce_parts(ws, grid.x, part, dkernels, stream);
-  scratch_free(ws, stream);
-  if (rc) return rc;
-  cdna_apply_bwd_dimage_kernel<<<grid, 256, 0, as_stream(stream)>>>(kernels, d_a, d_a_cstride, d_b, d_b_cstride, dimage, n, h, w, kh, kw, nk);
-  return check_launch("cdna_apply_bwd_dimage_kernel");
+  return vp_cdna_slots_bwd(&image, 1, kernels, nk, nk, d_a, d_a_cstride, d_b, d_b_cstride, &dimage, dkernels, n, h, w, kh, kw, stream);
 }
 
 extern "C" int vp_cdna_kernel_norm_bwd(const float* raw, const float* out, const float* dout, float* draw, int b, int kh, int kw,

@@ -44,6 +44,12 @@ int slab_gates_bwd(const float* pre, int n, int P, int F, const float* c_prev, c
                    const float* b2, const float* stats1, const float* stats2, float forget_bias, const float* const* dh, const int* dh_cs,
                    int num_dh, const float* dc_next, float* dpre, float* dc_prev, float* dg1, float* db1, float* dg2, float* db2,
                    vp_stream_t stream);
+// Device pointers of one slot-writer call, passed by value (__grid_constant__): ptr[f] = history frame f (oldest first),
+// ptr[VP_SLOT_MAX_FRAMES + b] = background b.  Backward calls pass the per-frame gradients the same way.
+struct VpSlotTable { const float* ptr[VP_SLOT_MAX_FRAMES + VP_SLOT_MAX_LAYERS]; };
+// Fills a table from the host arrays of a slot-writer call after checking nk, the frame split and the pointers (elementwise.cu).
+int slot_table(VpSlotTable* tab, const float* const* frames, int nframes, int nk, const float* const* backgrounds, int nbg,
+               const char* what);
 inline int grid_for(long long n, int block) { return static_cast<int>((n + block - 1) / block); }
 // Streaming multiprocessors of the current device (sizes persistent and split grids).
 inline int device_sms() {

@@ -398,11 +398,14 @@ __device__ __forceinline__ int reflect_idx(int i, int n) {  // SYMMETRIC padding
   if (i >= n) i = 2 * n - 1 - i;
   return i;
 }
-// image [N,H,W,4]; kern [N, KH*KW, NK]; writes NK transformed images + prev image + first image as
-// float4 slots into the masks-conv concat buffer: layers[n,y,x, off + 4*l .. ] (l = 0..NK+1).
-__global__ void __launch_bounds__(256) cdna_apply_kernel(const float4* __restrict__ image, const float4* __restrict__ first,
-                                                         const float* __restrict__ kern, float* __restrict__ layers,
-                                                         int ls, int N, int H, int W, int KH, int KW, int NK) {
+// Slot writer (savp_model.py:574-596, apply_cdna_kernels :893-923): frames [NF][N,H,W,4] are the history images oldest
+// first, kern [N, KH*KW, NK] their NK kernels, the k-th of which applies to frame k / (NK / NF).  Writes the NK transformed
+// images and then the NBG background images as float4 slots into the masks-conv concat buffer: layers[n,y,x, 4*l .. ].
+// kMaxNk bounds NK; the 4-slot instantiation is the default model's.
+template <int kMaxNk>
+__global__ void __launch_bounds__(256) cdna_slots_kernel(const __grid_constant__ VpSlotTable tab, const float* __restrict__ kern,
+                                                         float* __restrict__ layers, int ls, int N, int H, int W, int KH, int KW,
+                                                         int NK, int NF, int NBG) {
   extern __shared__ float sk[];  // [KH*KW*NK]
   const int n = blockIdx.y;
   for (int i = threadIdx.x; i < KH * KW * NK; i += blockDim.x) sk[i] = kern[static_cast<long long>(n) * KH * KW * NK + i];
@@ -410,38 +413,44 @@ __global__ void __launch_bounds__(256) cdna_apply_kernel(const float4* __restric
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= H * W) return;
   const int y = p / W, x = p % W;
-  const float4* img = image + static_cast<long long>(n) * H * W;
-  float4 acc[4];
+  const long long row = static_cast<long long>(n) * H * W;
+  const int G = NK ? NK / NF : 0;  // transforms per frame
+  float4 acc[kMaxNk];
 #pragma unroll
-  for (int k = 0; k < 4; ++k) acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = 0; k < kMaxNk; ++k) acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
   const int ph = (KH - 1) / 2, pw = (KW - 1) / 2;  // SAME pad-before for stride 1
-  for (int i = 0; i < KH; ++i) {
+  for (int i = 0; i < KH && NK; ++i) {
     const int yy = reflect_idx(y + i - ph, H);
     for (int j = 0; j < KW; ++j) {
       const int xx = reflect_idx(x + j - pw, W);
-      const float4 v = img[yy * W + xx];
       const float* kk = sk + (i * KW + j) * NK;
+      for (int f = 0; f < NF; ++f) {
+        const float4 v = reinterpret_cast<const float4*>(tab.ptr[f])[row + yy * W + xx];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (k < NK) {
-          acc[k].x += v.x * kk[k]; acc[k].y += v.y * kk[k]; acc[k].z += v.z * kk[k]; acc[k].w += v.w * kk[k];
+        for (int k = 0; k < kMaxNk; ++k) {
+          if (k < NK && k >= f * G && k < (f + 1) * G) {
+            acc[k].x += v.x * kk[k]; acc[k].y += v.y * kk[k]; acc[k].z += v.z * kk[k]; acc[k].w += v.w * kk[k];
+          }
         }
       }
     }
   }
-  float* lp = layers + (static_cast<long long>(n) * H * W + p) * ls;
-  for (int k = 0; k < NK; ++k) *reinterpret_cast<float4*>(lp + 4 * k) = acc[k];
-  *reinterpret_cast<float4*>(lp + 4 * NK) = img[p];
-  *reinterpret_cast<float4*>(lp + 4 * NK + 4) = first[static_cast<long long>(n) * H * W + p];
+  float* lp = layers + (row + p) * ls;
+#pragma unroll
+  for (int k = 0; k < kMaxNk; ++k)
+    if (k < NK) *reinterpret_cast<float4*>(lp + 4 * k) = acc[k];
+  for (int b = 0; b < NBG; ++b)
+    *reinterpret_cast<float4*>(lp + 4 * (NK + b)) = reinterpret_cast<const float4*>(tab.ptr[VP_SLOT_MAX_FRAMES + b])[row + p];
 }
 
-// logits [N*P, lgs] (L valid) ; layers: L float4 slots at layers[np*ls + 4*l] ; masks out [N*P, 8];
-// gen [N*P] float4 = sum_l softmax(logits)_l * layer_l
+// logits [N*P, lgs] (L valid) ; layers: L float4 slots at layers[np*ls + 4*l] ; masks out [N*P, ms];
+// gen [N*P] float4 = sum_l softmax(logits)_l * layer_l.  kMaxL bounds L; the 8-slot instantiation is the default model's.
+template <int kMaxL>
 __global__ void composite_kernel(const float* __restrict__ logits, int lgs, const float* __restrict__ layers, int ls,
                                  float* __restrict__ masks, int ms, float4* __restrict__ gen, long long total, int L) {
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= total) return;
-  float lg[8];
+  float lg[kMaxL];
   float mx = -1e30f;
   for (int l = 0; l < L; ++l) { lg[l] = logits[idx * lgs + l]; mx = fmaxf(mx, lg[l]); }
   float s = 0.f;
@@ -595,23 +604,66 @@ extern "C" int vp_cdna_kernel_norm(const float* raw, float* out, int b, int kh, 
   return check_launch("cdna_kernel_norm_kernel");
 }
 
+namespace vp {
+int slot_table(VpSlotTable* tab, const float* const* frames, int nframes, int nk, const float* const* backgrounds, int nbg,
+               const char* what) {
+  if (nk < 0 || nk > VP_SLOT_MAX_TRANSFORMS || nbg < 0 || nk + nbg > VP_SLOT_MAX_LAYERS)
+    return set_error("%s: bad nk / backgrounds (nk <= %d, nk + backgrounds <= %d)", what, VP_SLOT_MAX_TRANSFORMS, VP_SLOT_MAX_LAYERS);
+  if (nk && (nframes < 1 || nframes > VP_SLOT_MAX_FRAMES || nk % nframes))
+    return set_error("%s: the %d transforms must split evenly over 1..%d frames, got %d", what, nk, VP_SLOT_MAX_FRAMES, nframes);
+  if ((nk && !frames) || (nbg && !backgrounds)) return set_error("%s: null pointer", what);
+  *tab = VpSlotTable{};
+  for (int f = 0; nk && f < nframes; ++f) {
+    if (!frames[f]) return set_error("%s: null frame %d", what, f);
+    tab->ptr[f] = frames[f];
+  }
+  for (int b = 0; b < nbg; ++b) {
+    if (!backgrounds[b]) return set_error("%s: null background %d", what, b);
+    tab->ptr[VP_SLOT_MAX_FRAMES + b] = backgrounds[b];
+  }
+  return 0;
+}
+}  // namespace vp
+
+extern "C" int vp_cdna_slots(const float* const* frames, int nframes, const float* kernels, int nk, const float* const* backgrounds,
+                             int nbg, float* layers, int layers_cstride, int n, int h, int w, int kh, int kw, vp_stream_t stream) {
+  VpSlotTable tab;
+  if (slot_table(&tab, frames, nframes, nk, backgrounds, nbg, "vp_cdna_slots")) return -1;
+  if (!layers || (nk && !kernels)) return set_error("vp_cdna_slots: null pointer");
+  if (layers_cstride % 4 || layers_cstride < 4 * (nk + nbg)) return set_error("vp_cdna_slots: layers stride must be a multiple of 4 >= 4 * slots");
+  if (n < 1 || h < 1 || w < 1 || n > 65535 || (nk && (kh < 1 || kw < 1))) return set_error("vp_cdna_slots: bad n / h / w / kernel");
+  dim3 grid((h * w + 255) / 256, n);
+  const size_t smem = static_cast<size_t>(kh) * kw * nk * sizeof(float);
+  if (nk <= 4)
+    cdna_slots_kernel<4><<<grid, 256, smem, as_stream(stream)>>>(tab, kernels, layers, layers_cstride, n, h, w, kh, kw, nk, nframes, nbg);
+  else
+    cdna_slots_kernel<VP_SLOT_MAX_TRANSFORMS><<<grid, 256, smem, as_stream(stream)>>>(tab, kernels, layers, layers_cstride, n, h, w, kh,
+                                                                                        kw, nk, nframes, nbg);
+  return check_launch("cdna_slots_kernel");
+}
+
 extern "C" int vp_cdna_apply(const float* image, const float* first_image, const float* kernels, float* layers,
                              int layers_cstride, int n, int h, int w, int kh, int kw, int nk, vp_stream_t stream) {
   if (nk > 4) return set_error("vp_cdna_apply: at most 4 transformations");
   if (layers_cstride % 4) return set_error("vp_cdna_apply: layers stride must be a multiple of 4");
-  dim3 grid((h * w + 255) / 256, n);
-  cdna_apply_kernel<<<grid, 256, kh * kw * nk * sizeof(float), as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(image), reinterpret_cast<const float4*>(first_image), kernels, layers, layers_cstride, n,
-      h, w, kh, kw, nk);
-  return check_launch("cdna_apply_kernel");
+  const float* bg[2] = {image, first_image};
+  return vp_cdna_slots(&image, 1, kernels, nk, bg, 2, layers, layers_cstride, n, h, w, kh, kw, stream);
 }
 
 extern "C" int vp_composite(const float* logits, int logits_cstride, const float* layers, int layers_cstride, float* masks,
                             int masks_cstride, float* gen_image, long long positions, int num_layers, vp_stream_t stream) {
-  if (num_layers > 8) return set_error("vp_composite: at most 8 layers");
-  composite_kernel<<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(logits, logits_cstride, layers, layers_cstride, masks,
-                                                                           masks_cstride, reinterpret_cast<float4*>(gen_image),
-                                                                           positions, num_layers);
+  if (num_layers < 1 || num_layers > VP_SLOT_MAX_LAYERS)
+    return set_error("vp_composite: 1 .. %d layers, got %d", VP_SLOT_MAX_LAYERS, num_layers);
+  if (!logits || !layers || !gen_image) return set_error("vp_composite: null pointer");
+  if (logits_cstride < num_layers || (masks && masks_cstride < num_layers) || layers_cstride < 4 * num_layers)
+    return set_error("vp_composite: strides smaller than the %d layers", num_layers);
+  if (num_layers <= 8)
+    composite_kernel<8><<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(logits, logits_cstride, layers, layers_cstride, masks,
+                                                                              masks_cstride, reinterpret_cast<float4*>(gen_image),
+                                                                              positions, num_layers);
+  else
+    composite_kernel<VP_SLOT_MAX_LAYERS><<<grid_for(positions, 256), 256, 0, as_stream(stream)>>>(
+        logits, logits_cstride, layers, layers_cstride, masks, masks_cstride, reinterpret_cast<float4*>(gen_image), positions, num_layers);
   return check_launch("composite_kernel");
 }
 
@@ -691,21 +743,23 @@ extern "C" int vp_image_warp_bwd(const float* im, int im_cstride, const float* f
 
 // ------------------------------------------------------------------------------------------------
 // transformation = 'flow' (savp_model.py:522-530, 577-578, 955-965): the transformed images are backward bilinear warps
-// of the previous image by NK predicted flow fields.  `flows` is the 3x3 flows-conv output [N,H,W,2*NK] reshaped by the
-// reference to [.., 2, NK]: channel k is the x-flow of transform k, channel NK + k its y-flow.  Writes the NK warped
-// images + the previous image + the first image as consecutive float4 slots of the masks-conv concat buffer (same slot
-// layout as cdna_apply_kernel).  flow_ops.image_warp semantics: floor, four neighbours clipped to the image.
+// of the history images by NK predicted flow fields.  `flows` is the 3x3 flows-conv output [N,H,W,2*NK] reshaped by the
+// reference to [.., 2, NK]: channel k is the x-flow of transform k, channel NK + k its y-flow; transform k warps frame
+// k / (NK / NF).  Writes the NK warped images and then the NBG background images as consecutive float4 slots of the
+// masks-conv concat buffer (the slot layout of cdna_slots_kernel).  flow_ops.image_warp semantics: floor, four neighbours
+// clipped to the image.
 // ------------------------------------------------------------------------------------------------
 namespace vp {
-__global__ void __launch_bounds__(256) flow_apply_kernel(const float4* __restrict__ image, const float4* __restrict__ first,
-                                                         const float* __restrict__ flows, int fs, float* __restrict__ layers, int ls,
-                                                         int N, int H, int W, int NK) {
+__global__ void __launch_bounds__(256) flow_slots_kernel(const __grid_constant__ VpSlotTable tab, const float* __restrict__ flows, int fs,
+                                                         float* __restrict__ layers, int ls, int N, int H, int W, int NK, int NF, int NBG) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= static_cast<long long>(N) * H * W) return;
   const int x = static_cast<int>(p % W), y = static_cast<int>((p / W) % H);
   const long long base = p - (static_cast<long long>(y) * W + x);
+  const int G = NK ? NK / NF : 1;
   float* lp = layers + p * ls;
   for (int k = 0; k < NK; ++k) {
+    const float4* image = reinterpret_cast<const float4*>(tab.ptr[k / G]);
     const float fx = flows[p * fs + k], fy = flows[p * fs + NK + k];
     const float flx = floorf(fx), fly = floorf(fy);
     const float xw = fx - flx, yw = fy - fly;
@@ -717,26 +771,31 @@ __global__ void __launch_bounds__(256) flow_apply_kernel(const float4* __restric
     *reinterpret_cast<float4*>(lp + 4 * k) = make_float4(wa * Ia.x + wb * Ib.x + wc * Ic.x + wd * Id.x, wa * Ia.y + wb * Ib.y + wc * Ic.y + wd * Id.y,
                                                           wa * Ia.z + wb * Ib.z + wc * Ic.z + wd * Id.z, wa * Ia.w + wb * Ib.w + wc * Ic.w + wd * Id.w);
   }
-  *reinterpret_cast<float4*>(lp + 4 * NK) = image[p];
-  *reinterpret_cast<float4*>(lp + 4 * NK + 4) = first[p];
+  for (int b = 0; b < NBG; ++b)
+    *reinterpret_cast<float4*>(lp + 4 * (NK + b)) = reinterpret_cast<const float4*>(tab.ptr[VP_SLOT_MAX_FRAMES + b])[p];
 }
 
-// gradients of flow_apply: dT_k = dA[slot k] + dB[slot k] (through the masks conv and through the compositing);
-// dimage += scatter of the bilinear weights (+ the previous-image slot NK); dflows (overwritten): only the fractional
+// gradients of flow_slots: dT_k = dA[slot k] + dB[slot k] (through the masks conv and through the compositing);
+// dframe_{k / G} += scatter of the bilinear weights (atomic), dframe_{NF-1} += the slot PREV (the previous image as a
+// background, none if PREV < 0); frames whose dframe is NULL take no gradient.  dflows (overwritten): only the fractional
 // weights carry a gradient (floor has none, flow_ops.py:27-34).
-__global__ void __launch_bounds__(256) flow_apply_bwd_kernel(const float4* __restrict__ image, const float* __restrict__ flows, int fs,
-                                                             const float* __restrict__ dA, int das, const float* __restrict__ dB,
-                                                             int dbs, float* __restrict__ dimage, float* __restrict__ dflows, int N,
-                                                             int H, int W, int NK) {
+__global__ void __launch_bounds__(256) flow_slots_bwd_kernel(const __grid_constant__ VpSlotTable tab, const __grid_constant__ VpSlotTable dtab,
+                                                             const float* __restrict__ flows, int fs, const float* __restrict__ dA, int das,
+                                                             const float* __restrict__ dB, int dbs, float* __restrict__ dflows, int N,
+                                                             int H, int W, int NK, int NF, int PREV) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= static_cast<long long>(N) * H * W) return;
   const int x = static_cast<int>(p % W), y = static_cast<int>((p / W) % H);
   const long long base = p - (static_cast<long long>(y) * W + x);
-  {
-    const float4 a = *reinterpret_cast<const float4*>(dA + p * das + 4 * NK), b = *reinterpret_cast<const float4*>(dB + p * dbs + 4 * NK);
+  const int G = NK ? NK / NF : 1;
+  if (PREV >= 0 && dtab.ptr[NF - 1]) {
+    float* dimage = const_cast<float*>(dtab.ptr[NF - 1]);
+    const float4 a = *reinterpret_cast<const float4*>(dA + p * das + 4 * PREV), b = *reinterpret_cast<const float4*>(dB + p * dbs + 4 * PREV);
     atomicAdd(dimage + p * 4 + 0, a.x + b.x); atomicAdd(dimage + p * 4 + 1, a.y + b.y); atomicAdd(dimage + p * 4 + 2, a.z + b.z);
   }
   for (int k = 0; k < NK; ++k) {
+    const float4* image = reinterpret_cast<const float4*>(tab.ptr[k / G]);
+    float* dimage = const_cast<float*>(dtab.ptr[k / G]);
     const float4 a = *reinterpret_cast<const float4*>(dA + p * das + 4 * k), b = *reinterpret_cast<const float4*>(dB + p * dbs + 4 * k);
     const float d[3] = {a.x + b.x, a.y + b.y, a.z + b.z};
     const float fx = flows[p * fs + k], fy = flows[p * fs + NK + k];
@@ -753,10 +812,12 @@ __global__ void __launch_bounds__(256) flow_apply_bwd_kernel(const float4* __res
     for (int c = 0; c < 3; ++c) {
       gx += d[c] * ((1.f - yw) * (vc[c] - va[c]) + yw * (vd[c] - vb[c]));
       gy += d[c] * ((1.f - xw) * (vb[c] - va[c]) + xw * (vd[c] - vc[c]));
-      atomicAdd(dimage + ia * 4 + c, d[c] * (1.f - xw) * (1.f - yw));
-      atomicAdd(dimage + ib * 4 + c, d[c] * (1.f - xw) * yw);
-      atomicAdd(dimage + ic * 4 + c, d[c] * xw * (1.f - yw));
-      atomicAdd(dimage + id * 4 + c, d[c] * xw * yw);
+      if (dimage) {
+        atomicAdd(dimage + ia * 4 + c, d[c] * (1.f - xw) * (1.f - yw));
+        atomicAdd(dimage + ib * 4 + c, d[c] * (1.f - xw) * yw);
+        atomicAdd(dimage + ic * 4 + c, d[c] * xw * (1.f - yw));
+        atomicAdd(dimage + id * 4 + c, d[c] * xw * yw);
+      }
     }
     dflows[p * fs + k] = gx;
     dflows[p * fs + NK + k] = gy;
@@ -764,22 +825,50 @@ __global__ void __launch_bounds__(256) flow_apply_bwd_kernel(const float4* __res
 }
 }  // namespace vp
 
+extern "C" int vp_flow_slots(const float* const* frames, int nframes, const float* flows, int flows_cstride, int nk,
+                             const float* const* backgrounds, int nbg, float* layers, int layers_cstride, int n, int h, int w,
+                             vp_stream_t stream) {
+  vp::VpSlotTable tab;
+  if (vp::slot_table(&tab, frames, nframes, nk, backgrounds, nbg, "vp_flow_slots")) return -1;
+  if (!layers || (nk && !flows)) return vp::set_error("vp_flow_slots: null pointer");
+  if (nk && flows_cstride < 2 * nk) return vp::set_error("vp_flow_slots: flows_cstride < 2 * nk");
+  if (layers_cstride % 4 || layers_cstride < 4 * (nk + nbg)) return vp::set_error("vp_flow_slots: layers stride must be a multiple of 4 >= 4 * slots");
+  if (n < 1 || h < 1 || w < 1) return vp::set_error("vp_flow_slots: bad n / h / w");
+  const long long total = static_cast<long long>(n) * h * w;
+  vp::flow_slots_kernel<<<vp::grid_for(total, 256), 256, 0, vp::as_stream(stream)>>>(tab, flows, flows_cstride, layers, layers_cstride,
+                                                                                     n, h, w, nk, nframes, nbg);
+  return vp::check_launch("flow_slots_kernel");
+}
+
+extern "C" int vp_flow_slots_bwd(const float* const* frames, int nframes, const float* flows, int flows_cstride, int nk, int prev_slot,
+                                 const float* d_a, int d_a_cstride, const float* d_b, int d_b_cstride, float* const* dframes,
+                                 float* dflows, int n, int h, int w, vp_stream_t stream) {
+  vp::VpSlotTable tab, dtab{};
+  if (vp::slot_table(&tab, frames, nframes, nk, nullptr, 0, "vp_flow_slots_bwd")) return -1;
+  if (nframes < 1 || nframes > VP_SLOT_MAX_FRAMES || !dframes) return vp::set_error("vp_flow_slots_bwd: bad frames / dframes");
+  if (!d_a || !d_b || (nk && (!flows || !dflows))) return vp::set_error("vp_flow_slots_bwd: null pointer");
+  if (nk && flows_cstride < 2 * nk) return vp::set_error("vp_flow_slots_bwd: flows_cstride < 2 * nk");
+  if (prev_slot >= VP_SLOT_MAX_LAYERS || prev_slot < -1 || (prev_slot >= 0 && prev_slot < nk))
+    return vp::set_error("vp_flow_slots_bwd: bad prev_slot %d", prev_slot);
+  if (d_a_cstride % 4 || d_b_cstride % 4) return vp::set_error("vp_flow_slots_bwd: gradient strides must be multiples of 4");
+  if (n < 1 || h < 1 || w < 1) return vp::set_error("vp_flow_slots_bwd: bad n / h / w");
+  for (int f = 0; f < nframes; ++f) dtab.ptr[f] = dframes[f];
+  const long long total = static_cast<long long>(n) * h * w;
+  vp::flow_slots_bwd_kernel<<<vp::grid_for(total, 256), 256, 0, vp::as_stream(stream)>>>(
+      tab, dtab, flows, flows_cstride, d_a, d_a_cstride, d_b, d_b_cstride, dflows, n, h, w, nk, nframes, prev_slot);
+  return vp::check_launch("flow_slots_bwd_kernel");
+}
+
 extern "C" int vp_flow_apply(const float* image, const float* first_image, const float* flows, int flows_cstride, float* layers,
                              int layers_cstride, int n, int h, int w, int nk, vp_stream_t stream) {
   if (nk < 1 || nk > 6 || flows_cstride < 2 * nk) return vp::set_error("vp_flow_apply: bad nk / flows_cstride");
-  const long long total = static_cast<long long>(n) * h * w;
-  vp::flow_apply_kernel<<<vp::grid_for(total, 256), 256, 0, vp::as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(image), reinterpret_cast<const float4*>(first_image), flows, flows_cstride, layers, layers_cstride,
-      n, h, w, nk);
-  return vp::check_launch("flow_apply_kernel");
+  const float* bg[2] = {image, first_image};
+  return vp_flow_slots(&image, 1, flows, flows_cstride, nk, bg, 2, layers, layers_cstride, n, h, w, stream);
 }
 
 extern "C" int vp_flow_apply_bwd(const float* image, const float* flows, int flows_cstride, const float* d_a, int d_a_cstride,
                                  const float* d_b, int d_b_cstride, float* dimage, float* dflows, int n, int h, int w, int nk,
                                  vp_stream_t stream) {
   if (nk < 1 || nk > 6 || flows_cstride < 2 * nk) return vp::set_error("vp_flow_apply_bwd: bad nk / flows_cstride");
-  const long long total = static_cast<long long>(n) * h * w;
-  vp::flow_apply_bwd_kernel<<<vp::grid_for(total, 256), 256, 0, vp::as_stream(stream)>>>(
-      reinterpret_cast<const float4*>(image), flows, flows_cstride, d_a, d_a_cstride, d_b, d_b_cstride, dimage, dflows, n, h, w, nk);
-  return vp::check_launch("flow_apply_bwd_kernel");
+  return vp_flow_slots_bwd(&image, 1, flows, flows_cstride, nk, nk, d_a, d_a_cstride, d_b, d_b_cstride, &dimage, dflows, n, h, w, stream);
 }

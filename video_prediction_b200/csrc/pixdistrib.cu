@@ -15,7 +15,6 @@ namespace vp {
 
 constexpr int kPixClusterCtas = 8;
 constexpr int kPixThreads = 256;
-constexpr int kPixMaxSlots = 8;  // the masks buffer holds at most 8 layers (vp_composite)
 
 __device__ __forceinline__ int pd_reflect(int i, int n) {  // SYMMETRIC padding (edge pixel repeated), as cdna_apply_kernel
   if (i < 0) i = -i - 1;
@@ -23,11 +22,16 @@ __device__ __forceinline__ int pd_reflect(int i, int n) {  // SYMMETRIC padding 
   return i;
 }
 
+// The slots of one step: transform k < NK of history map k / (NK / NF) (map NF - 1 = this step's selected map p, maps
+// f < NF - 1 = tab.ptr[f], earlier steps' selected maps), then background b < NBG = tab.ptr[VP_SLOT_MAX_FRAMES + b] or, when
+// that pointer is NULL, p itself, then p again in the scratch slot when SCRATCH.  kMaxSlots bounds NK + NBG + SCRATCH; the
+// 8-slot instantiation is the default model's.
+template <int kMaxSlots>
 __global__ void __cluster_dims__(kPixClusterCtas, 1, 1) __launch_bounds__(kPixThreads)
-pix_distrib_fwd_kernel(const int32_t* __restrict__ sel, const float* __restrict__ gt, const float* __restrict__ first, int gts,
+pix_distrib_fwd_kernel(const __grid_constant__ VpSlotTable tab, const int32_t* __restrict__ sel, const float* __restrict__ gt, int gts,
                        const float* __restrict__ prev, const float* __restrict__ kern, const float* __restrict__ flows, int fs,
                        const float* __restrict__ masks, int ms, float* __restrict__ gen, int gs, float* __restrict__ tr, int trs,
-                       int tr_slot, int H, int W, int KH, int KW, int NK) {
+                       int tr_slot, float* __restrict__ cur_out, int H, int W, int KH, int KW, int NK, int NF, int NBG, int SCRATCH) {
   extern __shared__ float sk[];  // [KH*KW*NK] CDNA kernels of this row
   __shared__ float s_warp[kPixThreads / 32];
   __shared__ float s_part;
@@ -44,46 +48,57 @@ pix_distrib_fwd_kernel(const int32_t* __restrict__ sel, const float* __restrict_
   const bool use_gt = prev == nullptr || sel[n] != 0;
   const float* src = use_gt ? gt + row * gts + d : prev + row * gs + d;
   const int ss = use_gt ? gts : gs;
+  const int G = NK ? NK / NF : 1;
+  const int nslots = NK + NBG + SCRATCH;
   const int ppc = (P + kPixClusterCtas - 1) / kPixClusterCtas;
   const int p_end = min(P, (rank + 1) * ppc);
   float acc = 0.f;
   for (int p = rank * ppc + threadIdx.x; p < p_end; p += blockDim.x) {
     const int y = p / W, x = p % W;
-    float slot[kPixMaxSlots];
-    if (kern) {  // apply_cdna_kernels (savp_model.py:893-923)
+    float slot[kMaxSlots];
+    if (kern) {  // apply_cdna_kernels (savp_model.py:893-923), group f on history map f (apply_kernels, :939-943)
       for (int k = 0; k < NK; ++k) slot[k] = 0.f;
       const int ph = (KH - 1) / 2, pw = (KW - 1) / 2;
       for (int i = 0; i < KH; ++i) {
         const int yy = pd_reflect(y + i - ph, H);
         for (int j = 0; j < KW; ++j) {
-          const float v = src[static_cast<long long>(yy * W + pd_reflect(x + j - pw, W)) * ss];
+          const long long q = yy * W + pd_reflect(x + j - pw, W);
           const float* kk = sk + (i * KW + j) * NK;
-          for (int k = 0; k < NK; ++k) slot[k] += v * kk[k];
+          for (int f = 0; f < NF; ++f) {
+            const float v = f == NF - 1 ? src[q * ss] : tab.ptr[f][(row + q) * gts + d];
+            for (int k = f * G; k < (f + 1) * G; ++k) slot[k] += v * kk[k];
+          }
         }
       }
     } else {  // apply_flows (savp_model.py:955-965), flow_ops.image_warp
       const float* fp = flows + (row + p) * fs;
       for (int k = 0; k < NK; ++k) {
+        const int f = k / G;
+        const float* m = f == NF - 1 ? src : tab.ptr[f] + row * gts + d;
+        const int mst = f == NF - 1 ? ss : gts;
         const float fx = fp[k], fy = fp[NK + k];
         const float flx = floorf(fx), fly = floorf(fy);
         const float xw = fx - flx, yw = fy - fly;
         const int x0 = min(max(x + static_cast<int>(flx), 0), W - 1), x1 = min(max(x + static_cast<int>(flx) + 1, 0), W - 1);
         const int y0 = min(max(y + static_cast<int>(fly), 0), H - 1), y1 = min(max(y + static_cast<int>(fly) + 1, 0), H - 1);
-        const float Ia = src[static_cast<long long>(y0 * W + x0) * ss], Ib = src[static_cast<long long>(y1 * W + x0) * ss];
-        const float Ic = src[static_cast<long long>(y0 * W + x1) * ss], Id = src[static_cast<long long>(y1 * W + x1) * ss];
+        const float Ia = m[static_cast<long long>(y0 * W + x0) * mst], Ib = m[static_cast<long long>(y1 * W + x0) * mst];
+        const float Ic = m[static_cast<long long>(y0 * W + x1) * mst], Id = m[static_cast<long long>(y1 * W + x1) * mst];
         slot[k] = (1.f - xw) * (1.f - yw) * Ia + (1.f - xw) * yw * Ib + xw * (1.f - yw) * Ic + xw * yw * Id;
       }
     }
-    // background slots (:606-621): previous map, first ground-truth map, and the previous map again in the scratch slot
+    // background slots (:606-621): ground-truth maps, or the selected map itself; the scratch slot takes the map too
     const float pv = src[static_cast<long long>(p) * ss];
-    slot[NK] = pv;
-    slot[NK + 1] = first[(row + p) * gts + d];
-    slot[NK + 2] = pv;
+    if (cur_out) cur_out[(row + p) * gts + d] = pv;
+    for (int b = 0; b < NBG; ++b) {
+      const float* bp = tab.ptr[VP_SLOT_MAX_FRAMES + b];
+      slot[NK + b] = bp ? bp[(row + p) * gts + d] : pv;
+    }
+    if (SCRATCH) slot[NK + NBG] = pv;
     // composite (:648-652) with the image path's softmax masks
     const float* mp = masks + (row + p) * ms;
     float* tp = tr + (row + p) * trs + d;
     float g = 0.f;
-    for (int l = 0; l < NK + 3; ++l) {
+    for (int l = 0; l < nslots; ++l) {
       tp[static_cast<long long>(l) * tr_slot] = slot[l];
       g += slot[l] * mp[l];
     }
@@ -113,6 +128,51 @@ pix_distrib_fwd_kernel(const int32_t* __restrict__ sel, const float* __restrict_
 
 }  // namespace vp
 
+extern "C" int vp_pix_slots_fwd(const int32_t* sel, const float* pix_gt, int pix_cstride, const float* gen_prev,
+                                const float* const* frames, int nframes, const float* kernels, const float* flows, int flows_cstride,
+                                int nk, const float* const* backgrounds, int nbg, int scratch, const float* masks, int masks_cstride,
+                                float* gen, int gen_cstride, float* transformed, int transformed_cstride, int slot_stride,
+                                float* cur_out, int n, int h, int w, int d, int kh, int kw, vp_stream_t stream) {
+  using namespace vp;
+  const int nslots = nk + nbg + (scratch ? 1 : 0);
+  if (nk < 0 || nk > VP_SLOT_MAX_TRANSFORMS || nbg < 0 || nslots < 1 || nslots > VP_SLOT_MAX_LAYERS)
+    return set_error("vp_pix_slots_fwd: bad nk / backgrounds (nk <= %d, 1 <= slots <= %d)", VP_SLOT_MAX_TRANSFORMS, VP_SLOT_MAX_LAYERS);
+  if (nk && (nframes < 1 || nframes > VP_SLOT_MAX_FRAMES || nk % nframes))
+    return set_error("vp_pix_slots_fwd: the %d transforms must split evenly over 1..%d maps, got %d", nk, VP_SLOT_MAX_FRAMES, nframes);
+  if (!pix_gt || !masks || !gen || !transformed) return set_error("vp_pix_slots_fwd: null pointer");
+  if (nk && (kernels == nullptr) == (flows == nullptr)) return set_error("vp_pix_slots_fwd: pass exactly one of kernels and flows");
+  if (!nk && (kernels || flows)) return set_error("vp_pix_slots_fwd: kernels / flows without transforms");
+  if (gen_prev && !sel) return set_error("vp_pix_slots_fwd: gen_prev needs sel");
+  if (masks_cstride < nslots) return set_error("vp_pix_slots_fwd: masks_cstride < %d slots", nslots);
+  if (flows && flows_cstride < 2 * nk) return set_error("vp_pix_slots_fwd: flows_cstride < 2 * nk");
+  if (kernels && (kh < 1 || kw < 1 || kh / 2 > h || kw / 2 > w)) return set_error("vp_pix_slots_fwd: kernel larger than the image");
+  if (n < 1 || h < 1 || w < 1 || d < 1 || n > 65535 || d > 65535) return set_error("vp_pix_slots_fwd: bad n / h / w / d");
+  if (pix_cstride % 4 || gen_cstride % 4 || transformed_cstride % 4 || slot_stride % 4)
+    return set_error("vp_pix_slots_fwd: channel strides must be multiples of 4");
+  if (pix_cstride < d || gen_cstride < d || slot_stride < d || static_cast<long long>(nslots - 1) * slot_stride + d > transformed_cstride)
+    return set_error("vp_pix_slots_fwd: channel strides too small for d");
+  if ((nk && nframes > 1 && !frames) || (nbg && !backgrounds)) return set_error("vp_pix_slots_fwd: null pointer");
+  VpSlotTable tab{};
+  for (int f = 0; nk && f < nframes - 1; ++f) {
+    if (!frames[f]) return set_error("vp_pix_slots_fwd: null map %d", f);
+    tab.ptr[f] = frames[f];
+  }
+  for (int b = 0; b < nbg; ++b) tab.ptr[VP_SLOT_MAX_FRAMES + b] = backgrounds[b];   // NULL: the step's selected map
+  const int nf = nk ? nframes : 1;
+  const dim3 grid(kPixClusterCtas, n, d);
+  const size_t smem = kernels ? static_cast<size_t>(kh) * kw * nk * sizeof(float) : 0;
+  if (nslots <= 8)
+    pix_distrib_fwd_kernel<8><<<grid, kPixThreads, smem, as_stream(stream)>>>(tab, sel, pix_gt, pix_cstride, gen_prev, kernels, flows,
+                                                                             flows_cstride, masks, masks_cstride, gen, gen_cstride,
+                                                                             transformed, transformed_cstride, slot_stride, cur_out, h, w,
+                                                                             kh, kw, nk, nf, nbg, scratch ? 1 : 0);
+  else
+    pix_distrib_fwd_kernel<VP_SLOT_MAX_LAYERS><<<grid, kPixThreads, smem, as_stream(stream)>>>(
+        tab, sel, pix_gt, pix_cstride, gen_prev, kernels, flows, flows_cstride, masks, masks_cstride, gen, gen_cstride, transformed,
+        transformed_cstride, slot_stride, cur_out, h, w, kh, kw, nk, nf, nbg, scratch ? 1 : 0);
+  return check_launch("pix_distrib_fwd_kernel");
+}
+
 extern "C" int vp_pix_distrib_fwd(const int32_t* sel, const float* pix_gt, const float* pix_first, int pix_cstride,
                                   const float* gen_prev, const float* kernels, const float* flows, int flows_cstride,
                                   const float* masks, int masks_cstride, float* gen, int gen_cstride, float* transformed,
@@ -121,20 +181,9 @@ extern "C" int vp_pix_distrib_fwd(const int32_t* sel, const float* pix_gt, const
   using namespace vp;
   if (!pix_gt || !pix_first || !masks || !gen || !transformed) return set_error("vp_pix_distrib_fwd: null pointer");
   if ((kernels == nullptr) == (flows == nullptr)) return set_error("vp_pix_distrib_fwd: pass exactly one of kernels and flows");
-  if (gen_prev && !sel) return set_error("vp_pix_distrib_fwd: gen_prev needs sel");
-  if (nk < 1 || nk + 3 > kPixMaxSlots || masks_cstride < nk + 3) return set_error("vp_pix_distrib_fwd: bad nk / masks_cstride");
-  if (flows && flows_cstride < 2 * nk) return set_error("vp_pix_distrib_fwd: flows_cstride < 2 * nk");
-  if (kernels && (kh < 1 || kw < 1 || kh / 2 > h || kw / 2 > w))
-    return set_error("vp_pix_distrib_fwd: kernel larger than the image");
-  if (n < 1 || h < 1 || w < 1 || d < 1 || n > 65535 || d > 65535) return set_error("vp_pix_distrib_fwd: bad n / h / w / d");
-  if (pix_cstride % 4 || gen_cstride % 4 || transformed_cstride % 4 || slot_stride % 4)
-    return set_error("vp_pix_distrib_fwd: channel strides must be multiples of 4");
-  if (pix_cstride < d || gen_cstride < d || slot_stride < d || static_cast<long long>(nk + 2) * slot_stride + d > transformed_cstride)
-    return set_error("vp_pix_distrib_fwd: channel strides too small for d");
-  const dim3 grid(kPixClusterCtas, n, d);
-  const size_t smem = kernels ? static_cast<size_t>(kh) * kw * nk * sizeof(float) : 0;
-  pix_distrib_fwd_kernel<<<grid, kPixThreads, smem, as_stream(stream)>>>(sel, pix_gt, pix_first, pix_cstride, gen_prev, kernels, flows,
-                                                                       flows_cstride, masks, masks_cstride, gen, gen_cstride,
-                                                                       transformed, transformed_cstride, slot_stride, h, w, kh, kw, nk);
-  return check_launch("pix_distrib_fwd_kernel");
+  if (nk < 1 || nk + 3 > 8 || masks_cstride < nk + 3) return set_error("vp_pix_distrib_fwd: bad nk / masks_cstride");
+  const float* bg[2] = {nullptr, pix_first};     // the selected map, the first ground-truth map; then the scratch slot
+  return vp_pix_slots_fwd(sel, pix_gt, pix_cstride, gen_prev, nullptr, 1, kernels, flows, flows_cstride, nk, bg, 2, 1, masks,
+                          masks_cstride, gen, gen_cstride, transformed, transformed_cstride, slot_stride, nullptr, n, h, w, d, kh, kw,
+                          stream);
 }

@@ -375,6 +375,40 @@ def flow_apply_bwd(image, flows, flows_cs, da_addr, da_cs, db_addr, db_cs, dimag
                                   ptr(dflows), n, h, w, nk, stream_ptr()))
 
 
+SLOT_MAX_TRANSFORMS, SLOT_MAX_FRAMES, SLOT_MAX_LAYERS = 16, 16, 32     # VP_SLOT_MAX_* of vp_b200.h
+
+
+def _ptrs(addrs):
+    return (C.c_void_p * max(len(addrs), 1))(*[C.c_void_p(a or None) for a in addrs])
+
+
+def slots(frames, nk, backgrounds, layers_addr, layers_cs, n, h, w, kernels=None, kh=0, kw=0, flows=None, flows_cs=0):
+    """The slot writer (vp_cdna_slots, or vp_flow_slots when `flows` is given): nk transforms of the history frames, then the
+    background images, as float4 slots at layers_addr.  frames / backgrounds: lists of device addresses ([n][h][w][4] each)."""
+    if 'cdna' in _SKIP:
+        return
+    if flows is not None:
+        check(lib().vp_flow_slots(_ptrs(frames), len(frames), ptr(flows), flows_cs, nk, _ptrs(backgrounds), len(backgrounds),
+                                  addr(layers_addr), layers_cs, n, h, w, stream_ptr()))
+    else:
+        check(lib().vp_cdna_slots(_ptrs(frames), len(frames), ptr(kernels), nk, _ptrs(backgrounds), len(backgrounds),
+                                  addr(layers_addr), layers_cs, n, h, w, kh, kw, stream_ptr()))
+
+
+def slots_bwd(frames, nk, prev_slot, da_addr, da_cs, db_addr, db_cs, dframes, n, h, w, kernels=None, dkernels=None, kh=0, kw=0,
+              flows=None, flows_cs=0, dflows=None):
+    """Backward of `slots`: dframes (device addresses, 0 = no gradient) += each frame's gradient (+ slot prev_slot for the last
+    frame); dkernels += (CDNA) or dflows = (flow)."""
+    if 'cdna' in _SKIP:
+        return
+    if flows is not None:
+        check(lib().vp_flow_slots_bwd(_ptrs(frames), len(frames), ptr(flows), flows_cs, nk, prev_slot, addr(da_addr), da_cs,
+                                      addr(db_addr), db_cs, _ptrs(dframes), ptr(dflows), n, h, w, stream_ptr()))
+    else:
+        check(lib().vp_cdna_slots_bwd(_ptrs(frames), len(frames), ptr(kernels), nk, prev_slot, addr(da_addr), da_cs, addr(db_addr),
+                                      db_cs, _ptrs(dframes), ptr(dkernels), n, h, w, kh, kw, stream_ptr()))
+
+
 def composite(logits, logits_cs, layers_addr, layers_cs, masks, masks_cs, gen, positions, num_layers):
     if 'cdna' in _SKIP:
         return
@@ -389,6 +423,16 @@ def pix_distrib_fwd(sel, pix_gt_addr, pix_first_addr, pix_cs, gen_prev_addr, ker
     check(lib().vp_pix_distrib_fwd(ptr(sel), C.c_void_p(pix_gt_addr), C.c_void_p(pix_first_addr), pix_cs, C.c_void_p(gen_prev_addr),
                                    ptr(kernels), ptr(flows), flows_cs, ptr(masks), masks_cs, C.c_void_p(gen_addr), gen_cs,
                                    C.c_void_p(tr_addr), tr_cs, slot_stride, n, h, w, d, kh, kw, nk, stream_ptr()))
+
+
+def pix_slots_fwd(sel, pix_gt_addr, pix_cs, gen_prev_addr, frames, nk, backgrounds, scratch, masks, masks_cs, gen_addr, gen_cs,
+                  tr_addr, tr_cs, slot_stride, cur_out_addr, n, h, w, d, kernels=None, kh=0, kw=0, flows=None, flows_cs=0):
+    """One time step of the pixel-distribution path for any slot layout (vp_pix_slots_fwd): frames = the earlier steps'
+    selected maps (addresses, oldest first), backgrounds = ground-truth map addresses or 0 for the step's selected map."""
+    check(lib().vp_pix_slots_fwd(ptr(sel), addr(pix_gt_addr), pix_cs, addr(gen_prev_addr), _ptrs(frames), len(frames) + 1,
+                                 ptr(kernels), ptr(flows), flows_cs, nk, _ptrs(backgrounds), len(backgrounds), int(scratch), ptr(masks),
+                                 masks_cs, addr(gen_addr), gen_cs, addr(tr_addr), tr_cs, slot_stride, addr(cur_out_addr), n, h, w, d,
+                                 kh, kw, stream_ptr()))
 
 
 def state_pred_fwd(sel, states, states_stride, kernel, bias, zvec, zvec_stride, gen_states, s, n, a, sd):

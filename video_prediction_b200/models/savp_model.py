@@ -263,11 +263,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 raise ValueError('Invalid %s layer %s' % (key, getattr(hp, key + '_layer')))
         unsupported = []
         for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('last_frames', 1),
-                          ('prev_image_background', True), ('first_image_background', True),
-                          ('last_image_background', False), ('last_context_image_background', False),
-                          ('context_images_background', False), ('generate_scratch_image', True),
-                          ('dependent_mask', True), ('use_e_rnn', False), ('learn_prior', False),
+                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('use_e_rnn', False), ('learn_prior', False),
                           ('learn_initial_state', False), ('ablation_rnn', False),
                           ('use_rnn_z', True), ('joint_gan_optimization', False), ('use_same_discriminator', False)):
             # (`repeat` is accepted with any value: train.py sets it to the dataset's time_shift (train.py:160) and no model
@@ -287,6 +283,16 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                              "'none'")   # the reference calls None(h) (savp_model.py:380-383)
         if hp.transformation not in ('cdna', 'flow'):
             unsupported.append('transformation=%r' % (hp.transformation,))
+        # the compositing stage (savp_model.py:239-246, 561-653): L = num_masks slots, the first nk of them transforms
+        if hp.last_frames < 0 or hp.num_transformed_images < 0:
+            unsupported.append('last_frames=%r, num_transformed_images=%r' % (hp.last_frames, hp.num_transformed_images))
+        comp = self.compositing(hp)
+        if not comp['L']:       # savp_model.py:641-644
+            raise ValueError('Either one of the following should be true: last_frames and num_transformed_images, '
+                             'first_image_background, prev_image_background, generate_scratch_image')
+        if comp['nk'] > L.SLOT_MAX_TRANSFORMS or comp['L'] > L.SLOT_MAX_LAYERS:
+            unsupported.append('last_frames * num_transformed_images=%d (at most %d) with %d compositing layers (at most %d)'
+                               % (comp['nk'], L.SLOT_MAX_TRANSFORMS, comp['L'], L.SLOT_MAX_LAYERS))
         if tuple(hp.dilation_rate) != (1, 1):
             unsupported.append('dilation_rate=%r' % (hp.dilation_rate,))
         if self.mode == 'train':
@@ -300,6 +306,23 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 unsupported.append('kl_anneal=%r' % (hp.kl_anneal,))
         if unsupported:
             raise NotImplementedError('hparams outside the H100 hot path (SURVEY.md 8f): ' + ', '.join(unsupported))
+
+    @staticmethod
+    def compositing(hp):
+        """The slot layout of the compositing stage (savp_model.py:239-246, 574-596): nk transforms of the F most recent
+        images (F = last_frames, oldest first; none unless last_frames and num_transformed_images), then the backgrounds in
+        the reference's order -- 'prev' (the step's input image), 'first' (images[0]), 'last' (images[context_frames-1]),
+        'last_context' (images[min(t, context_frames-1)]), ('context', i) (images[i], i < context_frames) -- then the
+        scratch image.  L = every slot; masks exist only for L > 1."""
+        nk = hp.last_frames * hp.num_transformed_images if (hp.last_frames and hp.num_transformed_images) else 0
+        ctx = hp.context_images_background
+        bgs = (['prev'] if hp.prev_image_background else []) + (['first'] if hp.first_image_background and not ctx else []) + \
+              (['last'] if hp.last_image_background and not ctx else []) + \
+              (['last_context'] if hp.last_context_image_background and not ctx else []) + \
+              ([('context', i) for i in range(hp.context_frames)] if ctx else [])
+        scratch = bool(hp.generate_scratch_image)
+        return dict(nk=nk, F=hp.last_frames if nk else 1, bgs=bgs, scratch=scratch, L=nk + len(bgs) + int(scratch),
+                    prev_slot=nk + bgs.index('prev') if 'prev' in bgs else -1)
 
     @property
     def cell_norm(self):
@@ -421,28 +444,31 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             outs.append(oc)
         nl = n_enc + len(dec)
         kh, kw = hp.kernel_size
-        nk = hp.last_frames * hp.num_transformed_images
+        comp = self.compositing(hp)
+        nk, nlayers = comp['nk'], comp['L']
         sh = H // (2 ** n_enc)
         sw = W // (2 ** n_enc)
         top = outs[-1]
-        if hp.transformation == 'flow':         # savp_model.py:522-530: flow heads instead of the CDNA kernel dense layer
+        if nk and hp.transformation == 'flow':     # savp_model.py:522-530: flow heads instead of the CDNA kernel dense layer
             specs['%s/h%d_flow/conv2d/kernel' % (sc, nl)] = ((3, 3, top, hp.ngf), 'kernel')
             specs['%s/h%d_flow/conv2d/bias' % (sc, nl)] = ((hp.ngf,), 'zeros')
             site_norm('%s/h%d_flow' % (sc, nl), hp.ngf)
             specs[sc + '/flows/conv2d/kernel'] = ((3, 3, hp.ngf, 2 * nk), 'kernel')
             specs[sc + '/flows/conv2d/bias'] = ((2 * nk,), 'zeros')
-        else:
+        elif nk:
             specs[sc + '/cdna_kernels/dense/kernel'] = ((sh * sw * outs[n_enc - 1], kh * kw * nk), 'kernel')
             specs[sc + '/cdna_kernels/dense/bias'] = ((kh * kw * nk,), 'zeros')
-        for nm in ('h%d_scratch' % nl, 'h%d_masks' % nl):
+        heads = (['h%d_scratch' % nl] if comp['scratch'] else []) + (['h%d_masks' % nl] if nlayers > 1 else [])
+        for nm in heads:
             specs['%s/%s/conv2d/kernel' % (sc, nm)] = ((3, 3, top, hp.ngf), 'kernel')
             specs['%s/%s/conv2d/bias' % (sc, nm)] = ((hp.ngf,), 'zeros')
             site_norm('%s/%s' % (sc, nm), hp.ngf)
-        specs[sc + '/scratch_image/conv2d/kernel'] = ((3, 3, hp.ngf, C), 'kernel')
-        specs[sc + '/scratch_image/conv2d/bias'] = ((C,), 'zeros')
-        nlayers = nk + 3
-        specs[sc + '/masks/conv2d/kernel'] = ((3, 3, hp.ngf + nlayers * C, nlayers), 'kernel')
-        specs[sc + '/masks/conv2d/bias'] = ((nlayers,), 'zeros')
+        if comp['scratch']:
+            specs[sc + '/scratch_image/conv2d/kernel'] = ((3, 3, hp.ngf, C), 'kernel')
+            specs[sc + '/scratch_image/conv2d/bias'] = ((C,), 'zeros')
+        if nlayers > 1:     # dependent_mask: the masks conv also reads every slot (savp_model.py:630-633)
+            specs[sc + '/masks/conv2d/kernel'] = ((3, 3, hp.ngf + (nlayers * C if hp.dependent_mask else 0), nlayers), 'kernel')
+            specs[sc + '/masks/conv2d/bias'] = ((nlayers,), 'zeros')
         if self.Sd:       # savp_model.py:655-658: the next robot state from [actions | state]
             specs[sc + '/state_pred/dense/kernel'] = ((A + self.Sd, self.Sd), 'kernel')
             specs[sc + '/state_pred/dense/bias'] = ((self.Sd,), 'zeros')
@@ -843,27 +869,39 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         self.nl = nl
         top = outs[-1]
         kh, kw = hp.kernel_size
-        nk = hp.last_frames * hp.num_transformed_images
+        self.comp = comp = self.compositing(hp)
+        nk = comp['nk']
         self.nk, self.kh, self.kw = nk, kh, kw
-        self.nlayers = nk + 3
-        sl = self.gl[n_enc - 1]
-        Bf['small'] = self._z(S, NB, sl['h'] * sl['w'] * sl['oc'])
-        Bf['kraw'] = self._z(S, NB, kh * kw * nk)
-        Bf['kern'] = self._z(S, NB, kh * kw * nk)
+        self.nlayers = comp['L']
+        self.flow = hp.transformation == 'flow' and nk > 0      # the flow heads
+        self.cdna = hp.transformation == 'cdna' and nk > 0      # the CDNA kernel dense layer
+        if self.cdna:
+            sl = self.gl[n_enc - 1]
+            Bf['small'] = self._z(S, NB, sl['h'] * sl['w'] * sl['oc'])
+            Bf['kraw'] = self._z(S, NB, kh * kw * nk)
+            Bf['kern'] = self._z(S, NB, kh * kw * nk)
         top_spec = ConcatSpec([('x', top)])
         self.top_spec = top_spec
-        self.conv_scratch = ConvLayer(self, '%s/h%d_scratch/conv2d/kernel' % (sc, nl), '%s/h%d_scratch/conv2d/bias' % (sc, nl),
-                                      (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
-        self.conv_hmasks = ConvLayer(self, '%s/h%d_masks/conv2d/kernel' % (sc, nl), '%s/h%d_masks/conv2d/bias' % (sc, nl),
-                                     (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
         hs_spec = ConcatSpec([('x', hp.ngf)])
-        self.conv_simg = ConvLayer(self, sc + '/scratch_image/conv2d/kernel', sc + '/scratch_image/conv2d/bias',
-                                   (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, hs_spec, C)
+        # the masks-conv input: h_masks, then the L slots (the scratch image last)
         self.mk_spec = ConcatSpec([('hm', hp.ngf)] + [('l%d' % l, C) for l in range(self.nlayers)])
-        self.conv_masks = ConvLayer(self, sc + '/masks/conv2d/kernel', sc + '/masks/conv2d/bias', (1, 3, 3), L.WKIND_PLAIN,
-                                    (1, 1, 1), (0, 1, 1), False, self.mk_spec, self.nlayers)
-        self.convs += [self.conv_scratch, self.conv_hmasks, self.conv_simg, self.conv_masks]
-        self.flow = hp.transformation == 'flow'
+        self.conv_scratch = self.conv_hmasks = self.conv_simg = self.conv_masks = None
+        if comp['scratch']:
+            self.conv_scratch = ConvLayer(self, '%s/h%d_scratch/conv2d/kernel' % (sc, nl), '%s/h%d_scratch/conv2d/bias' % (sc, nl),
+                                          (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
+        if self.nlayers > 1:
+            self.conv_hmasks = ConvLayer(self, '%s/h%d_masks/conv2d/kernel' % (sc, nl), '%s/h%d_masks/conv2d/bias' % (sc, nl),
+                                         (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
+        if comp['scratch']:
+            self.conv_simg = ConvLayer(self, sc + '/scratch_image/conv2d/kernel', sc + '/scratch_image/conv2d/bias',
+                                       (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, hs_spec, C)
+        if self.nlayers > 1:
+            # independent masks read h_masks alone: the slot channels of the buffer get zero weights (cmap -1)
+            msp = self.mk_spec
+            mspec = msp if hp.dependent_mask else (hp.ngf, msp.cstride, list(range(hp.ngf)) + [-1] * (msp.cstride - hp.ngf))
+            self.conv_masks = ConvLayer(self, sc + '/masks/conv2d/kernel', sc + '/masks/conv2d/bias', (1, 3, 3), L.WKIND_PLAIN,
+                                        (1, 1, 1), (0, 1, 1), False, mspec, self.nlayers)
+        self.convs += [c for c in (self.conv_scratch, self.conv_hmasks, self.conv_simg, self.conv_masks) if c is not None]
         if self.flow:
             self.conv_hflow = ConvLayer(self, '%s/h%d_flow/conv2d/kernel' % (sc, nl), '%s/h%d_flow/conv2d/bias' % (sc, nl),
                                         (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
@@ -880,8 +918,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         Bf['mst'] = self._norm_stats(S, NB, hp.ngf)
         Bf['hs'] = self._z(S, NB, H, W, hp.ngf)
         Bf['mk'] = self._z(S, NB, H, W, self.mk_spec.cstride)
-        Bf['mlog'] = self._z(S, NB, H, W, 8)
-        Bf['masks'] = self._z(S, NB, H, W, 8)
+        self.mc = max(8, _ceil4(self.nlayers))     # channel stride of the mask logits and masks
+        Bf['mlog'] = self._z(S, NB, H, W, self.mc)
+        Bf['masks'] = self._z(S, NB, H, W, self.mc)
         Bf['gen'] = self._z(S, NB, H, W, 4)
         Bf['img'] = self._z(S, NB, H, W, 4)
         Bf['x'] = self._z(self.T, NB, H, W, 4)
@@ -893,6 +932,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             Bf['pix'] = self._z(self.T, NB, H, W, Dp)
             Bf['gpix'] = self._z(S, NB, H, W, Dp)
             Bf['tpix'] = self._z(S, NB, H, W, self.nlayers * Dp)
+            if self.comp['F'] > 1:      # the selected map of every step: the history of the later steps' transforms
+                Bf['ppix'] = self._z(S, NB, H, W, Dp)
         if Zc:
             Bf['zvec'] = self._z(S, NB, _ceil4(Zc))
         if self.Sd:
@@ -1202,7 +1243,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             i = n_enc - 1 - li
             sp = self.gl[n_enc + i]['in_spec']
             dests.append((Bf['in%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
-        if li == n_enc - 1 and not self.flow:     # flattened input of the CDNA kernel dense layer
+        if li == n_enc - 1 and self.cdna:     # flattened input of the CDNA kernel dense layer
             dests.append((Bf['small'][t].data_ptr(), d['oc']))
         return dests
 
@@ -1266,7 +1307,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             self._site_norm('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act, 0.0,
                             Bf['fst'][t])
             self.conv_flows.fwd(Bf['hf'][t], Bf['flows'][t], out_c=2 * nk)
-        else:
+        elif self.cdna:
             # cdna kernels (savp_model.py:546-559)
             small = Bf['small'][t]
             K = small.shape[1]
@@ -1277,33 +1318,61 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         # heads
         mk = Bf['mk'][t]
         msp = self.mk_spec
-        self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t], act=self.site_act)
-        self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'), act=self.site_act)
-        self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act, 0.0,
-                        Bf['sst'][t])
-        self._site_norm('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
-                        self.site_act, 0.0, Bf['mst'][t])
-        # scratch image -> last layer slot (savp_model.py:570-572, 595-596)
-        self.conv_simg.fwd(Bf['hs'][t], mk, out_off=msp.off('l%d' % (self.nlayers - 1)), out_c=C, act=L.ACT_SIGMOID)
-        # transformed images: 4 CDNA (or flow-warped) + prev image + first image (savp_model.py:574-584)
-        if self.flow:
-            L.flow_apply(Bf['img'][t], Bf['x'][0], Bf['flows'][t], Bf['flows'].shape[-1], mk.data_ptr() + 4 * msp.off('l0'),
-                         msp.cstride, NB, H, W, nk)
-        else:
-            L.cdna_apply(Bf['img'][t], Bf['x'][0], Bf['kern'][t], mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, NB, H, W,
-                         kh, kw, nk)
-        # masks + compositing (savp_model.py:623-646)
-        self.conv_masks.fwd(mk, Bf['mlog'][t], out_c=self.nlayers)
-        L.composite(Bf['mlog'][t], 8, mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, Bf['masks'][t], 8, Bf['gen'][t],
+        if self.conv_scratch:
+            self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t], act=self.site_act)
+        if self.conv_hmasks:
+            self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'), act=self.site_act)
+        if self.conv_scratch:
+            self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act,
+                            0.0, Bf['sst'][t])
+        if self.conv_hmasks:
+            self._site_norm('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
+                            self.site_act, 0.0, Bf['mst'][t])
+        if self.conv_simg:      # scratch image -> last layer slot (savp_model.py:570-572, 595-596)
+            self.conv_simg.fwd(Bf['hs'][t], mk, out_off=msp.off('l%d' % (self.nlayers - 1)), out_c=C, act=L.ACT_SIGMOID)
+        # transformed images of the history, then the backgrounds (savp_model.py:574-594)
+        frames, _ = self._history(t)
+        L.slots(frames, nk, self._backgrounds(t), mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, NB, H, W,
+                kernels=Bf['kern'][t] if self.cdna else None, kh=kh, kw=kw, flows=Bf['flows'][t] if self.flow else None,
+                flows_cs=Bf['flows'].shape[-1] if self.flow else 0)
+        # masks + compositing (savp_model.py:623-646); a single layer has the mask 1 = softmax of one zero logit
+        if self.conv_masks:
+            self.conv_masks.fwd(mk, Bf['mlog'][t], out_c=self.nlayers)
+        L.composite(Bf['mlog'][t], self.mc, mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, Bf['masks'][t], self.mc, Bf['gen'][t],
                     NB * HW, self.nlayers)
         if self.D:
             # pixel distributions (savp_model.py:408-410, 598-621, 648-653): same selection, transformation and masks
+            # the same slots from the maps (savp_model.py:598-621): history maps for the transforms, ground-truth maps or
+            # the step's selected map (0) as backgrounds
             Dp = Bf['gpix'].shape[-1]
-            L.pix_distrib_fwd(Bf['sel'][t], Bf['pix'][t].data_ptr(), Bf['pix'][0].data_ptr(), Dp,
-                              Bf['gpix'][t - 1].data_ptr() if t else 0, None if self.flow else Bf['kern'][t],
-                              Bf['flows'][t] if self.flow else None, Bf['flows'].shape[-1] if self.flow else 0,
-                              Bf['masks'][t], 8, Bf['gpix'][t].data_ptr(), Dp, Bf['tpix'][t].data_ptr(), self.nlayers * Dp, Dp,
-                              NB, H, W, self.D, kh, kw, nk)
+            pix, ppix = Bf['pix'], Bf.get('ppix')
+            hist = [(ppix[s] if s >= 0 else pix[0]).data_ptr() for s in range(t - self.comp['F'] + 1, t)]
+            bgs = [0 if b == 'prev' else a for b, a in zip(self.comp['bgs'], self._backgrounds(t, pix))]
+            L.pix_slots_fwd(Bf['sel'][t], pix[t].data_ptr(), Dp, Bf['gpix'][t - 1].data_ptr() if t else 0, hist, nk, bgs,
+                            self.comp['scratch'], Bf['masks'][t], self.mc, Bf['gpix'][t].data_ptr(), Dp, Bf['tpix'][t].data_ptr(),
+                            self.nlayers * Dp, Dp, ppix[t].data_ptr() if ppix is not None else 0, NB, H, W, self.D,
+                            kernels=Bf['kern'][t] if self.cdna else None, kh=kh, kw=kw,
+                            flows=Bf['flows'][t] if self.flow else None, flows_cs=Bf['flows'].shape[-1] if self.flow else 0)
+
+    def _history(self, t):
+        """(device addresses, gradient addresses) of the F images the transforms of step t read, oldest first
+        (savp_model.py:349-351, 407): img_s for s = t-F+1 .. t, the first ground-truth image for s < 0, which takes no
+        gradient."""
+        Bf = self.Bf
+        F = self.comp['F']
+        frames, dframes = [], []
+        G = getattr(self, 'Gb', None)
+        for s in range(t - F + 1, t + 1):
+            frames.append(Bf['img'][s].data_ptr() if s >= 0 else Bf['x'][0].data_ptr())
+            dframes.append(G['dimg'][s].data_ptr() if (G is not None and s >= 0) else 0)
+        return frames, dframes
+
+    def _backgrounds(self, t, x=None):
+        """Device addresses of the background slots of step t, in slot order (savp_model.py:581-594), taken from the
+        ground-truth frames x (default the images) and, for 'prev', the step's input image."""
+        x, ctx = self.Bf['x'] if x is None else x, self.hparams.context_frames
+        src = {'prev': self.Bf['img'][t], 'first': x[0], 'last': x[ctx - 1], 'last_context': x[t if t < ctx else ctx - 1]}
+        return [(x[b[1]] if isinstance(b, tuple) else src[b]).data_ptr() for b in self.comp['bgs']]
 
     def generator_forward(self, collect=True):
         hp = self.hparams

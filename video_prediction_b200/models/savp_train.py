@@ -221,7 +221,7 @@ class TrainMixin(object):
         ngf = hp.ngf
         G['dgen'] = z(S, NB, H, W, 4)
         G['dimg'] = z(S, NB, H, W, 4)
-        G['dmlog'] = z(S, NB, H, W, 8)
+        G['dmlog'] = z(S, NB, H, W, self.mc)
         G['dlay'] = z(S, NB, H, W, 4 * self.nlayers)
         G['dmk'] = torch.zeros_like(Bf['mk'])
         G['dmpre'] = z(S, NB, H, W, ngf)
@@ -229,9 +229,10 @@ class TrainMixin(object):
         G['dsimg'] = z(S, NB, H, W, 4)
         G['dhs'] = z(S, NB, H, W, ngf)
         G['dtop'] = z(S, NB, H, W, self.gl[-1]['oc'])
-        G['dkern'] = torch.zeros_like(Bf['kern'])
-        G['dkraw'] = torch.zeros_like(Bf['kraw'])
-        G['dsmall'] = torch.zeros_like(Bf['small'])
+        if self.cdna:
+            G['dkern'] = torch.zeros_like(Bf['kern'])
+            G['dkraw'] = torch.zeros_like(Bf['kraw'])
+            G['dsmall'] = torch.zeros_like(Bf['small'])
         if self.flow:
             G['dflows'] = torch.zeros_like(Bf['flows'])
             G['dhf'] = z(S, NB, H, W, ngf)
@@ -331,44 +332,57 @@ class TrainMixin(object):
         msp = self.mk_spec
         mk, dmk = Bf['mk'][t], G['dmk'][t]
         nlay = self.nlayers
-        # compositing + masks conv
-        L.composite_bwd(G['dgen'][t], Bf['masks'][t], 8, mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, G['dmlog'][t], 8,
-                        G['dlay'][t], 4 * nlay, NB * HW, nlay)
-        self.conv_masks.dgrad(G['dmlog'][t], dmk, dy_c=nlay)
-        # h_masks branch
-        self._site_norm_bwd('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride,
-                            [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, self.site_act, 0.0,
-                            Bf['mst'][t])
-        self.conv_hmasks.dgrad(G['dmpre'][t], G['dtop'][t])
-        # scratch branch
-        so = msp.off('l%d' % (nlay - 1))
-        L.act_bwd(mk.data_ptr() + 4 * so, msp.cstride, dmk.data_ptr() + 4 * so, msp.cstride,
-                  G['dlay'][t].data_ptr() + 4 * 4 * (nlay - 1), 4 * nlay, G['dsimg'][t].data_ptr(), 4, NB * HW, C, L.ACT_SIGMOID)
-        self.conv_simg.dgrad(G['dsimg'][t], G['dhs'][t], dy_c=C)
-        self._site_norm_bwd('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, [(G['dhs'][t].data_ptr(), ngf)],
-                            G['dspre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['sst'][t])
-        self.conv_scratch.dgrad(G['dspre'][t], G['dtop'][t], accumulate=True)
+        # compositing + masks conv; with a single layer (mask 1) nothing reaches the masks conv and dmk stays zero
+        L.composite_bwd(G['dgen'][t], Bf['masks'][t], self.mc, mk.data_ptr() + 4 * msp.off('l0'), msp.cstride, G['dmlog'][t],
+                        self.mc, G['dlay'][t], 4 * nlay, NB * HW, nlay)
+        dtop_acc = False       # the first head gradient overwrites dtop, the others add
+        if self.conv_masks:
+            self.conv_masks.dgrad(G['dmlog'][t], dmk, dy_c=nlay)
+            # h_masks branch
+            self._site_norm_bwd('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride,
+                                [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, self.site_act, 0.0,
+                                Bf['mst'][t])
+            self.conv_hmasks.dgrad(G['dmpre'][t], G['dtop'][t])
+            dtop_acc = True
+        if self.conv_scratch:
+            # scratch branch
+            so = msp.off('l%d' % (nlay - 1))
+            L.act_bwd(mk.data_ptr() + 4 * so, msp.cstride, dmk.data_ptr() + 4 * so, msp.cstride,
+                      G['dlay'][t].data_ptr() + 4 * 4 * (nlay - 1), 4 * nlay, G['dsimg'][t].data_ptr(), 4, NB * HW, C, L.ACT_SIGMOID)
+            self.conv_simg.dgrad(G['dsimg'][t], G['dhs'][t], dy_c=C)
+            self._site_norm_bwd('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf,
+                                [(G['dhs'][t].data_ptr(), ngf)], G['dspre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['sst'][t])
+            self.conv_scratch.dgrad(G['dspre'][t], G['dtop'][t], accumulate=dtop_acc)
+            dtop_acc = True
         nk, kh, kw = self.nk, self.kh, self.kw
-        G['dimg'][t].zero_()
+        # transforms and the previous-image background -> the history images (dimg[s], zeroed once per backward, so that
+        # the later steps' contributions are already in dimg[t] when step t propagates it)
+        frames, dframes = self._history(t)
+        da = (dmk.data_ptr() + 4 * msp.off('l0'), msp.cstride, G['dlay'][t].data_ptr(), 4 * nlay)
         if self.flow:
             # flow warps (flow_ops.py:4-79) -> flows conv -> h_flow instance norm -> h_flow conv (savp_model.py:522-530)
-            L.flow_apply_bwd(Bf['img'][t], Bf['flows'][t], Bf['flows'].shape[-1], dmk.data_ptr() + 4 * msp.off('l0'), msp.cstride,
-                             G['dlay'][t].data_ptr(), 4 * nlay, G['dimg'][t], G['dflows'][t], NB, H, W, nk)
+            L.slots_bwd(frames, nk, self.comp['prev_slot'], *da, dframes, NB, H, W, flows=Bf['flows'][t], flows_cs=Bf['flows'].shape[-1],
+                        dflows=G['dflows'][t])
             self.conv_flows.dgrad(G['dflows'][t], G['dhf'][t], dy_c=2 * nk)
             self._site_norm_bwd('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, [(G['dhf'][t].data_ptr(), ngf)],
                                 G['dfpre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['fst'][t])
-            self.conv_hflow.dgrad(G['dfpre'][t], G['dtop'][t], accumulate=True)
+            self.conv_hflow.dgrad(G['dfpre'][t], G['dtop'][t], accumulate=dtop_acc)
+            dtop_acc = True
+        elif not self.cdna:
+            L.slots_bwd(frames, 0, self.comp['prev_slot'], *da, dframes, NB, H, W)
         else:
             # CDNA
             G['dkern'][t].zero_()
-            L.cdna_apply_bwd(Bf['img'][t], Bf['kern'][t], dmk.data_ptr() + 4 * msp.off('l0'), msp.cstride, G['dlay'][t].data_ptr(),
-                             4 * nlay, G['dimg'][t], G['dkern'][t], NB, H, W, kh, kw, nk)
+            L.slots_bwd(frames, nk, self.comp['prev_slot'], *da, dframes, NB, H, W, kernels=Bf['kern'][t], dkernels=G['dkern'][t],
+                        kh=kh, kw=kw)
             L.cdna_kernel_norm_bwd(Bf['kraw'][t], Bf['kern'][t], G['dkern'][t], G['dkraw'][t], NB, kh, kw, nk)
             K = Bf['small'].shape[-1]
             dn = sc + '/cdna_kernels/dense'
             # dx only; dW / dbias of this layer are one GEMM over all time steps in _gen_backward_params
             L.dense_bwd(Bf['small'][t], K, P[dn + '/kernel'], G['dkraw'][t], kh * kw * nk, NB, K, kh * kw * nk, dx=G['dsmall'][t],
                         dx_stride=K)
+        if not dtop_acc:        # no head reads the top layer
+            G['dtop'][t].zero_()
         # encoder/decoder stack in reverse
         n_enc = len(self.enc_specs)
         for li in range(nl - 1, -1, -1):
@@ -384,7 +398,7 @@ class TrainMixin(object):
                 i = n_enc - 1 - li
                 sp = self.gl[n_enc + i]['in_spec']
                 srcs.append((G['din%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
-            if li == n_enc - 1 and not self.flow:
+            if li == n_enc - 1 and self.cdna:
                 srcs.append((G['dsmall'][t].data_ptr(), oc))
             if d['use'] and not self.cell_norm:
                 rsp = d['rin_spec']
@@ -461,20 +475,24 @@ class TrainMixin(object):
                 done.append((lo, hi))
         top = Bf['out%d' % (self.nl - 1)]
         ngf = hp.ngf
-        self.conv_scratch.wgrad(top, G['dspre'])
-        L.colsum(G['dspre'].data_ptr(), ngf, Gp[self.conv_scratch.bname], 1, rows_top, ngf)
-        self.conv_hmasks.wgrad(top, G['dmpre'])
-        L.colsum(G['dmpre'].data_ptr(), ngf, Gp[self.conv_hmasks.bname], 1, rows_top, ngf)
-        self.conv_simg.wgrad(Bf['hs'], G['dsimg'], dy_c=C)
-        L.colsum(G['dsimg'].data_ptr(), 4, Gp[self.conv_simg.bname], 1, rows_top, C)
-        self.conv_masks.wgrad(Bf['mk'], G['dmlog'], dy_c=self.nlayers)
-        L.colsum(G['dmlog'].data_ptr(), 8, Gp[self.conv_masks.bname], 1, rows_top, self.nlayers)
+        if self.conv_scratch:
+            self.conv_scratch.wgrad(top, G['dspre'])
+            L.colsum(G['dspre'].data_ptr(), ngf, Gp[self.conv_scratch.bname], 1, rows_top, ngf)
+        if self.conv_hmasks:
+            self.conv_hmasks.wgrad(top, G['dmpre'])
+            L.colsum(G['dmpre'].data_ptr(), ngf, Gp[self.conv_hmasks.bname], 1, rows_top, ngf)
+        if self.conv_simg:
+            self.conv_simg.wgrad(Bf['hs'], G['dsimg'], dy_c=C)
+            L.colsum(G['dsimg'].data_ptr(), 4, Gp[self.conv_simg.bname], 1, rows_top, C)
+        if self.conv_masks:
+            self.conv_masks.wgrad(Bf['mk'], G['dmlog'], dy_c=self.nlayers)
+            L.colsum(G['dmlog'].data_ptr(), self.mc, Gp[self.conv_masks.bname], 1, rows_top, self.nlayers)
         if self.flow:
             self.conv_hflow.wgrad(top, G['dfpre'])
             L.colsum(G['dfpre'].data_ptr(), ngf, Gp[self.conv_hflow.bname], 1, rows_top, ngf)
             self.conv_flows.wgrad(Bf['hf'], G['dflows'], dy_c=2 * self.nk)
             L.colsum(G['dflows'].data_ptr(), G['dflows'].shape[-1], Gp[self.conv_flows.bname], 1, rows_top, 2 * self.nk)
-        else:
+        elif self.cdna:
             # CDNA kernel dense layer: dW = sum over all time steps of small_t^T dkraw_t, one launch
             Kd = Bf['small'].shape[-1]
             dn = 'generator/rnn/savp_cell/cdna_kernels/dense'
@@ -720,6 +738,7 @@ class TrainMixin(object):
                 L.scatter_clip(net['dclip'][B:], net['ts'][('d_post', 1)], G['dgen'], B, net['clip_len'], HW, NB, foff)
             self._run_concurrent([(lambda sc=sc, nt=nt: g_step_tower(sc, nt)) for sc, nt in self.dnets.items()])
         # ---- BPTT
+        G['dimg'].zero_()
         for t in range(S - 1, -1, -1):
             self._gen_backward_step(t)
         self._gen_backward_params(red)

@@ -298,8 +298,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if self.mode == 'train':
             # loss terms of base_model.py:733-852 that are not built: refuse instead of silently dropping them
             for key in ('vgg_cdist_weight', 'feature_l2_weight', 'ae_l2_weight', 'state_weight', 'tv_weight', 'z_l1_weight',
-                        'images_sn_gan_weight', 'images_sn_vae_gan_weight', 'gan_feature_l2_weight',
-                        'vae_gan_feature_l2_weight'):
+                        'gan_feature_l2_weight', 'vae_gan_feature_l2_weight'):
                 if getattr(hp, key):
                     unsupported.append('%s=%r' % (key, getattr(hp, key)))
             if hp.kl_weight and hp.kl_anneal not in ('none', 'sigmoid', 'linear'):

@@ -25,16 +25,22 @@ VIDEO_D_LAYERS = [  # networks.py:83-102: (scope, ndf multiplier, kernel, stride
     ('sn_conv3_0', 8, 3, (1, 1, 1)),
 ]
 IMAGE_D_LAYERS = [  # networks.py:45-63 (image_sn_discriminator): the 2-D analogue, applied to ONE sampled frame per video
+                    # (kind 'image') or to every frame of the clip (kind 'images', through tf_utils.with_flat_batch)
     ('sn_conv0_0', 1, 3, (1, 1, 1)), ('sn_conv0_1', 2, 4, (1, 2, 2)),
     ('sn_conv1_0', 2, 3, (1, 1, 1)), ('sn_conv1_1', 4, 4, (1, 2, 2)),
     ('sn_conv2_0', 4, 3, (1, 1, 1)), ('sn_conv2_1', 8, 4, (1, 2, 2)),
     ('sn_conv3_0', 8, 3, (1, 1, 1)),
 ]
 
-LOSS_SLOTS = ['gen_l1_loss', 'gen_l2_loss', 'gen_kl_loss']
-for _kind in ('video', 'image'):
-    LOSS_SLOTS += ['gen_%s_sn_gan_loss' % _kind, 'gen_%s_sn_vae_gan_loss' % _kind, 'gen_%s_sn_vae_gan_feature_cdist_loss' % _kind,
-                   'gen_%s_sn_gan_feature_cdist_loss' % _kind, 'discrim_%s_sn_gan_loss' % _kind, 'discrim_%s_sn_vae_gan_loss' % _kind]
+
+def _gan_slots(kind):
+    return ['gen_%s_sn_gan_loss' % kind, 'gen_%s_sn_vae_gan_loss' % kind, 'gen_%s_sn_vae_gan_feature_cdist_loss' % kind,
+            'gen_%s_sn_gan_feature_cdist_loss' % kind, 'discrim_%s_sn_gan_loss' % kind, 'discrim_%s_sn_vae_gan_loss' % kind]
+
+
+# the loss terms every training model reports; a model with the per-frame `images` towers reports their six after these
+LOSS_SLOTS = ['gen_l1_loss', 'gen_l2_loss', 'gen_kl_loss'] + _gan_slots('video') + _gan_slots('image')
+IMAGES_LOSS_SLOTS = _gan_slots('images')
 
 
 def _ceil4(v):
@@ -119,12 +125,14 @@ class TrainMixin(object):
         """Discriminator towers of discriminator_fn / discriminator_given_video_fn (savp_model.py:88-166): per enabled kind
         (image: one sampled frame, networks.py:35-69; video: a clip_length clip, networks.py:72-108) one tower in the root
         scope (real / fake = prior-unroll images) and, with nz > 0, one with separate weights under encoder/ (enc_real /
-        enc_fake = posterior-unroll images; use_same_discriminator=False).  `images_sn_*` (per-frame discriminator over the
-        whole clip) is refused in _check_supported."""
+        enc_fake = posterior-unroll images; use_same_discriminator=False).  The `images` kind (the image discriminator on
+        every frame of the video tower's clip, savp_model.py:120-126) comes last, so that adding it moves neither the
+        variables nor the per-tower random draws of the other two."""
         hp = self.hparams
         towers = []
         for kind, w_gan, w_vae in (('image', hp.image_sn_gan_weight, hp.image_sn_vae_gan_weight),
-                                   ('video', hp.video_sn_gan_weight, hp.video_sn_vae_gan_weight)):
+                                   ('video', hp.video_sn_gan_weight, hp.video_sn_vae_gan_weight),
+                                   ('images', hp.images_sn_gan_weight, hp.images_sn_vae_gan_weight)):
             if w_gan or w_vae:
                 if hp.nz:
                     towers.append(dict(scope='discriminator/encoder/' + kind, kind=kind, enc=True, weight=w_vae,
@@ -136,11 +144,20 @@ class TrainMixin(object):
     def _d_scopes(self):
         return [t['scope'] for t in self._d_towers()]
 
+    def _d_clip_len(self, kind):
+        """Frames per sample a tower reads: the clip (video, images) or the one sampled frame (image)."""
+        return 1 if kind == 'image' else self.hparams.clip_length
+
+    def _d_frames(self, kind):
+        """Logits per sample: one per clip frame for the per-frame `images` tower, else one."""
+        return self.hparams.clip_length if kind == 'images' else 1
+
     def _d_shapes(self, kind='video'):
-        """Output dims (T',H',W',C') of the 7 conv layers for clips [clip,H,W,C] (image towers: clip = 1, no temporal taps)."""
+        """Output dims (T',H',W',C') of the 7 conv layers for clips [clip,H,W,C] (2-D towers: no temporal taps, T' = clip
+        for `images`, 1 for `image`)."""
         hp = self.hparams
         layers = VIDEO_D_LAYERS if kind == 'video' else IMAGE_D_LAYERS
-        dims = (hp.clip_length if kind == 'video' else 1, self.H, self.W)
+        dims = (self._d_clip_len(kind), self.H, self.W)
         out = []
         for name, mult, k, st in layers:
             kk, pad = ((k, k, k), (1, 1, 1)) if kind == 'video' else ((1, k, k), (0, 1, 1))
@@ -164,7 +181,7 @@ class TrainMixin(object):
                 specs['%s/%s/%s/u' % (scope, name, sub)] = ((1, co), 'u')
                 specs['%s/%s/%s/bias' % (scope, name, sub)] = ((co,), 'zeros')
                 cin = co
-            f = int(np.prod(shapes[-1]))
+            f = int(np.prod(shapes[-1])) // self._d_frames(kind)     # the images tower's dense reads one frame per row
             specs['%s/sn_fc4/dense/kernel' % scope] = ((f, 1), 'kernel')
             specs['%s/sn_fc4/dense/u' % scope] = ((1, 1), 'u')
             specs['%s/sn_fc4/dense/bias' % scope] = ((1,), 'zeros')
@@ -180,25 +197,27 @@ class TrainMixin(object):
             scope, kind = tw['scope'], tw['kind']
             shapes = self._d_shapes(kind)
             layers = VIDEO_D_LAYERS if kind == 'video' else IMAGE_D_LAYERS
-            clip_len = hp.clip_length if kind == 'video' else 1
-            net = dict(tw, layers=[], feat=[], dfeat=[], dcd=[], clip_len=clip_len)
+            # images: the 2-D layers' (1, k, k) kernels over a depth-clip input are the per-frame convolution, and the final
+            # dense has one row per frame (2B * clip logits)
+            clip_len, frames = self._d_clip_len(kind), self._d_frames(kind)
+            net = dict(tw, layers=[], feat=[], dfeat=[], dcd=[], clip_len=clip_len, frames=frames)
             spec = (C, 4, list(range(C)) + [-1] * (4 - C))      # colour channels stored as float4 voxels
             nb = 2 * B
             net['clip'] = z(nb, clip_len, H, W, 4)
             net['dclip'] = z(nb, clip_len, H, W, 4)
             for (name, mult, k, st), shp in zip(layers, shapes):
                 co = hp.ndf * mult
-                net['layers'].append(SNLayer(self, scope, name, k, st, spec, co, two_d=(kind == 'image')))
+                net['layers'].append(SNLayer(self, scope, name, k, st, spec, co, two_d=(kind != 'video')))
                 net['feat'].append(z(nb, *shp))
                 net['dfeat'].append(z(nb, *shp))
                 net['dcd'].append(z(B, *shp))
                 spec = (co, co, None)
-            f = int(np.prod(shapes[-1]))
+            f = int(np.prod(shapes[-1])) // frames
             net['fc'] = SNLayer(self, scope, 'sn_fc4', 1, None, None, 1, is_fc=True, fc_in=f)
             # every weight pack of the tower in one launch, run after the tower's spectral-norm forwards wrote sigma
             net['pack'] = L.PackPlan([job for lay in net['layers'] for job in lay.conv.pack_jobs()])
-            net['logits'] = z(nb)
-            net['dlogits'] = z(nb)
+            net['logits'] = z(nb * frames)
+            net['dlogits'] = z(nb * frames)
             net['tstart'] = torch.zeros(2, B, dtype=torch.int32, device=self.device)
             self.dnets[scope] = net
 
@@ -253,7 +272,7 @@ class TrainMixin(object):
                 G['depre%d' % i] = torch.zeros_like(Bf['epre%d' % i])
                 if i > 0:
                     G['deact%d' % i] = torch.zeros_like(Bf['eact%d' % i])
-        self.loss_vals = z(len(LOSS_SLOTS))
+        self.loss_vals = z(len(self.loss_slots()))
         self._graph, self._eager_steps = None, 0
         self.step_scalars = z(4)      # [lr_t(D), lr_t(G), kl_scale, -]  refreshed from the host every step
         self._scal_host = torch.zeros(4, dtype=torch.float32).pin_memory()
@@ -277,30 +296,31 @@ class TrainMixin(object):
         L.gather_clip(Bf['gen'], t_fake, net['clip'][B:], B, net['clip_len'], HW, NB, fake_off)
 
     def _d_forward(self, net, r0, r1):
-        """Runs the tower on clip rows [r0, r1)."""
+        """Runs the tower on clip rows [r0, r1) (logit rows [r0, r1) * frames)."""
         x = net['clip'][r0:r1]
         for lay, feat in zip(net['layers'], net['feat']):
             lay.fwd(x, feat[r0:r1])
             x = feat[r0:r1]
         fc = net['fc']
-        n = r1 - r0
-        net['logits'][r0:r1].zero_()
+        fr = net['frames']
+        logits = net['logits'][r0 * fr:r1 * fr]
+        logits.zero_()
         P = self.params
-        L.dense_fwd(x, fc.rows, P[fc.wname], P[fc.bname], net['logits'][r0:r1], 1, n, fc.rows, 1, k_splits=64,
-                    inv_scale=fc.sigma)
+        L.dense_fwd(x, fc.rows, P[fc.wname], P[fc.bname], logits, 1, (r1 - r0) * fr, fc.rows, 1, k_splits=64, inv_scale=fc.sigma)
 
     def _d_backward(self, net, r0, r1, with_wgrad, to_clip, dcd=None):
         """Back-propagates net['dlogits'][r0:r1] (and optional per-layer feature gradients dcd, rows [0, r1-r0))."""
         P, Gp = self.params, self.grads
         n = r1 - r0
         fc = net['fc']
+        fr = net['frames']
         feats, dfeats = net['feat'], net['dfeat']
-        last = feats[-1][r0:r1]
-        L.dense_bwd(last, fc.rows, P[fc.wname], net['dlogits'][r0:r1], 1, n, fc.rows, 1, dx=dfeats[-1][r0:r1], dx_stride=fc.rows,
+        last, dlogits = feats[-1][r0:r1], net['dlogits'][r0 * fr:r1 * fr]
+        L.dense_bwd(last, fc.rows, P[fc.wname], dlogits, 1, n * fr, fc.rows, 1, dx=dfeats[-1][r0:r1], dx_stride=fc.rows,
                     inv_scale=fc.sigma)
         if with_wgrad:
             fc.gwbar.zero_()
-            L.dense_bwd(last, fc.rows, P[fc.wname], net['dlogits'][r0:r1], 1, n, fc.rows, 1, dw=fc.gwbar, dbias=Gp[fc.bname])
+            L.dense_bwd(last, fc.rows, P[fc.wname], dlogits, 1, n * fr, fc.rows, 1, dw=fc.gwbar, dbias=Gp[fc.bname])
             fc.sn_backward()
         for l in range(len(feats) - 1, -1, -1):
             lay = net['layers'][l]
@@ -562,18 +582,31 @@ class TrainMixin(object):
             L.colsum(G['depre%d' % i].data_ptr(), oc, Gp[el['conv'].bname], 1, S * B * pos, oc)
 
     # ------------------------------------------------------------------ one optimisation step
+    def loss_slots(self):
+        """Names of the entries of loss_vals: LOSS_SLOTS, then IMAGES_LOSS_SLOTS when the images towers are built."""
+        hp = self.hparams
+        return LOSS_SLOTS + (IMAGES_LOSS_SLOTS if (hp.images_sn_gan_weight or hp.images_sn_vae_gan_weight) else [])
+
     def _slot(self, name):
-        return self.loss_vals[LOSS_SLOTS.index(name):LOSS_SLOTS.index(name) + 1]
+        i = self.loss_slots().index(name)
+        return self.loss_vals[i:i + 1]
 
     def _set_tstarts(self, noise):
         """Clip offsets t_start[B] in [0, T-1-clip_length] (video towers) / frame indices t_sample[B] in [0, T-2] (image towers)
         of the two discriminator_fn instantiations (pre / post D update; savp_model.py:93-98).  `noise[which][key]` (as the
-        oracle takes them: 'real', 'fake', 'enc_real', 'enc_fake' for video, 'image_*' for image towers) overrides the draw."""
+        oracle takes them: 'real', 'fake', 'enc_real', 'enc_fake' for video, 'image_*' for image towers) overrides the draw.
+        An `images` tower reads the same clip_sample as the video tower of its unroll (savp_model.py:97-102): it shares that
+        tower's offset buffers, and only draws its own (same range, same keys) when there is no video tower."""
         for ti, (scope, net) in enumerate(self.dnets.items()):
+            if net['kind'] == 'images':
+                video = self.dnets.get(scope[:-len('images')] + 'video')
+                if video is not None:
+                    net['ts'] = video['ts']
+                    continue
             hi = self.S - net['clip_len'] + 1
             for w, which in enumerate(('d_pre', 'd_post')):
                 for r, key in enumerate(net['keys']):
-                    nkey = key if net['kind'] == 'video' else 'image_' + key
+                    nkey = 'image_' + key if net['kind'] == 'image' else key
                     if noise is not None and which in noise and nkey in noise[which]:
                         v = torch.as_tensor(noise[which][nkey]).to(torch.int32)
                     else:
@@ -679,8 +712,9 @@ class TrainMixin(object):
                 self._d_gather(net, 'pre', net['ts'][('d_pre', 0)], net['ts'][('d_pre', 1)], 0 if enc else (B if hp.nz else 0))
                 self._d_forward(net, 0, 2 * B)
                 slot = self._slot('discrim_%s_sn_%sgan_loss' % (kind, 'vae_' if enc else ''))
-                L.gan_loss(net['logits'][:B], 1.0, B, w, hp.gan_loss_type, net['dlogits'][:B], slot)
-                L.gan_loss(net['logits'][B:], 0.0, B, w, hp.gan_loss_type, net['dlogits'][B:], slot)
+                n = B * net['frames']       # images: the mean over every frame's logit
+                L.gan_loss(net['logits'][:n], 1.0, n, w, hp.gan_loss_type, net['dlogits'][:n], slot)
+                L.gan_loss(net['logits'][n:], 0.0, n, w, hp.gan_loss_type, net['dlogits'][n:], slot)
                 self._d_backward(net, 0, 2 * B, with_wgrad=True, to_clip=False)
                 if red is not None:      # this tower's gradients are final: exchange them under the other towers' backward
                     lo, hi = self._flat_range(self.d_flat, [k for k in self.params if k.startswith(scope + '/') and not k.endswith('/u')])
@@ -721,7 +755,8 @@ class TrainMixin(object):
                 need_real = bool(cd_w)
                 self._d_gather(net, 'post', net['ts'][('d_post', 0)], net['ts'][('d_post', 1)], foff, rows_real=need_real)
                 self._d_forward(net, 0 if need_real else B, 2 * B)
-                L.gan_loss(net['logits'][B:], 1.0, B, w, hp.gan_loss_type, net['dlogits'][B:],
+                n = B * net['frames']
+                L.gan_loss(net['logits'][n:], 1.0, n, w, hp.gan_loss_type, net['dlogits'][n:],
                            self._slot('gen_%s_sn_%sgan_loss' % (kind, 'vae_' if enc else '')))
                 dcd = None
                 if cd_w:
@@ -733,10 +768,13 @@ class TrainMixin(object):
                         rows = int(np.prod(feat.shape[1:-1])) * B
                         L.cosine_distance(feat[B:], feat[:B], dcd[l], rows, co, cd_w, slot)
                 self._d_backward(net, B, 2 * B, with_wgrad=False, to_clip=True, dcd=dcd)
-                # the towers scatter into disjoint sample rows of dgen per unroll; towers of different kinds on the same
-                # unroll accumulate (scatter_clip adds)
-                L.scatter_clip(net['dclip'][B:], net['ts'][('d_post', 1)], G['dgen'], B, net['clip_len'], HW, NB, foff)
             self._run_concurrent([(lambda sc=sc, nt=nt: g_step_tower(sc, nt)) for sc, nt in self.dnets.items()])
+            # the towers of one unroll scatter into the same sample rows of dgen (scatter_clip adds): after the join and in
+            # tower order, so that the sum is the same on every run
+            for net in self.dnets.values():
+                if net['weight']:
+                    foff = 0 if net['enc'] else (B if hp.nz else 0)
+                    L.scatter_clip(net['dclip'][B:], net['ts'][('d_post', 1)], G['dgen'], B, net['clip_len'], HW, NB, foff)
         # ---- BPTT
         G['dimg'].zero_()
         for t in range(S - 1, -1, -1):
@@ -773,13 +811,17 @@ class TrainMixin(object):
         self.step_scalars.copy_(self._scal_host, non_blocking=True)
 
     def loss_weights(self, step=None):
-        """name -> weight of every loss slot at `step` (base_model.py:733-852; the KL weight is annealed, :312-319)."""
+        """name -> weight of every loss slot (loss_slots()) at `step` (base_model.py:733-852; the KL weight is annealed,
+        :312-319)."""
         hp = self.hparams
         step = self._staged_step if step is None else step
         kl = (self.kl_weight_at(step) or 0.0) if (hp.kl_weight and hp.nz) else 0.0
         w = OrderedDict([('gen_l1_loss', hp.l1_weight), ('gen_l2_loss', hp.l2_weight), ('gen_kl_loss', kl)])
         for kind, w_gan, w_vae in (('video', hp.video_sn_gan_weight, hp.video_sn_vae_gan_weight),
-                                   ('image', hp.image_sn_gan_weight, hp.image_sn_vae_gan_weight)):
+                                   ('image', hp.image_sn_gan_weight, hp.image_sn_vae_gan_weight),
+                                   ('images', hp.images_sn_gan_weight, hp.images_sn_vae_gan_weight)):
+            if kind == 'images' and not (w_gan or w_vae):
+                continue
             w['gen_%s_sn_gan_loss' % kind] = w_gan
             w['gen_%s_sn_vae_gan_loss' % kind] = w_vae if hp.nz else 0.0
             w['gen_%s_sn_vae_gan_feature_cdist_loss' % kind] = hp.vae_gan_feature_cdist_weight if (w_vae and hp.nz) else 0.0
@@ -805,6 +847,6 @@ class TrainMixin(object):
             from .. import dp
             dp.mean_scalars(lv)
         vals = lv.cpu().numpy()
-        out = OrderedDict((k, float(v)) for k, v in zip(LOSS_SLOTS, vals))
+        out = OrderedDict((k, float(v)) for k, v in zip(self.loss_slots(), vals))
         self.g_losses, self.d_losses, self.g_loss, self.d_loss = self.split_losses(out, self.loss_weights())
         return out

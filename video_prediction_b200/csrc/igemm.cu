@@ -133,7 +133,8 @@ __device__ __forceinline__ void lstm_store(const IgemmArgs& a, long long pix, co
 // forward / dgrad kernel.  A CTA owns one (BN-column tile, phase, k-split) and walks the 128-pixel tiles
 // m = blockIdx.x, blockIdx.x + gridDim.x, ... (persistent): the TMA ring keeps streaming across tiles, so the loads of
 // tile i+1 overlap the epilogue of tile i.  A ring stage is one 32-channel k-chunk: a 16 KB activation tile (128 rows)
-// and a BN x 128 B weight tile, both 128B-swizzled.
+// and a BN x 128 B weight tile, both 128B-swizzled.  One wgmma group per consumer stays in flight: a stage is released
+// once the group that read it has completed, while the next chunk's MMAs are already queued.
 // ------------------------------------------------------------------------------------------------
 constexpr int kFwdThreads = 384;
 template <int BN, bool kLstm, bool kElu = false>
@@ -220,12 +221,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int kq = it0 % a.kc;
+    uint32_t held = 0;     // empty barrier of the stage read by the wgmma group still in flight
 #pragma unroll 1
     for (int it = it0; it < it1; ++it) {
       mbar_wait_addr(full0 + b_off, ph);
       // the last k-chunk of a tap may hold fewer than 32 real channels (e.g. 72 = 32 + 32 + 8): the zero-filled K = 8
-      // slices are not multiplied at all
-      const int nk = kq == kq_last ? a.k_tail : 4;
+      // slices are not multiplied at all.  kq is the same in every thread, but only a vote makes that visible to ptxas:
+      // a wgmma behind a branch it cannot prove warp-uniform is serialised (a wait after every MMA, ptxas advisory C7520)
+      const int nk = __all_sync(0xffffffffu, kq == kq_last) ? a.k_tail : 4;
       const uint64_t ad = ad_base + adv, bd = bd_base + adv;
       wgmma_fence();
       Wgmma<BN>::mma(acc, ad, bd, 1u);
@@ -233,14 +236,21 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
       if (nk > 2) Wgmma<BN>::mma(acc, ad + 4, bd + 4, 1u);
       if (nk > 3) Wgmma<BN>::mma(acc, ad + 6, bd + 6, 1u);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_acc(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive_addr(empty0 + b_off);
+      // one group stays in flight: the previous chunk's group has completed, so its stage goes back to the producer
+      wgmma_wait<1>();
+      if (it > it0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive_addr(empty0 + held);
+      }
+      held = b_off;
       kq = kq == kq_last ? 0 : kq + 1;
       adv += kStageAdv; b_off += 8;
       if (b_off == ring_end) { b_off = 0; ph ^= 1; adv = 0; }
     }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive_addr(empty0 + held);
     int mt = mtile;
     const int tw = mt % a.tiles_w; mt /= a.tiles_w;
     const int th = mt % a.tiles_h; mt /= a.tiles_h;

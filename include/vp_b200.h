@@ -71,6 +71,14 @@ int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const float* wpack
                   const vp_tensor* out, const float* bias, int act, float alpha, int split_k, int accumulate,
                   vp_stream_t stream);
 
+/* The tile vp_conv_igemm and vp_conv_igemm_actgrad launch for a call of this shape on a device with `sms` SMs: `rows`
+ * output pixels x `bn` GEMM columns.  out_ndhw = the output's {n, d, h, w}; g, n_pad, kc and split_k as passed to the
+ * call.  It depends on the shape alone, so every call of one shape runs the same kernel. */
+int vp_conv_igemm_form(const vp_conv_geom* g, const int out_ndhw[4], int n_pad, int kc, int split_k, int sms, int* rows,
+                       int* bn);
+/* The tiles vp_conv_igemm_form can return, into rows[i], bn[i] for i < min(count, cap); returns the count. */
+int vp_conv_igemm_forms(int* rows, int* bn, int cap);
+
 /* Input-gradient convolution fused with the backward of the previous layer's activation:
  *   out = (conv(in) + addend) * act'(act_output),  act' evaluated from the activation OUTPUT (any VP_ACT_*);
  * act_output / addend (optional) have exactly the layout of the dense `out`.  Used for the discriminator towers

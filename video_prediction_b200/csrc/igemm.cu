@@ -5,15 +5,16 @@
 //
 // Operands are fp32 in HBM/shared memory and are consumed as TF32 by the tensor cores with fp32 accumulation in
 // registers.  Activation tiles are fetched with 5-D TMA boxes straight from the NDHWC tensor: a box of bw x bh x bd x bn
-// positions is one 128-row (64-row for the wgrad's dy) operand tile whose rows are 32 channels = 128 bytes, written by TMA
+// positions is one 128-row or 64-row operand tile whose rows are 32 channels = 128 bytes, written by TMA
 // with the 128-byte swizzle.  A filter tap is a coordinate shift of the box; TMA zero-fills out-of-bounds rows/channels,
 // which *is* the convolution's zero padding.  Strided convolutions read one of s_d*s_h*s_w "parity" sub-lattices of the
 // input (one tensor map each); transposed convolutions (upsample_conv2d forward, dgrad of strided convs) are split into
 // output phases.
 //
 // Forward / dgrad: both operands are K-major (channels contiguous), which is what wgmma needs for TF32: warpgroup 0 is
-// the TMA producer, warpgroups 1 and 2 each issue wgmma.m64nBNk8 on one 64-row half of the 128-pixel tile and run the
-// epilogue (bias / activation / fused activation gradient) from their accumulator registers.
+// the TMA producer, warpgroups 1 and 2 issue wgmma on one 64-row half each of a 128-pixel tile (m64nBNk8), or on one half
+// each of the columns of a 64-pixel tile (m64n(BN/2)k8), and run the epilogue (bias / activation / fused activation
+// gradient) from their accumulator registers.  Each call's tile is chosen from its shape (pick_fwd_form).
 // Weight gradient: GEMM-K is the pixel dimension, so both NDHWC operands are MN-major, which wgmma does not accept from
 // shared memory for TF32.  A pre-pass copies the un-shifted operand channel-major in tile order (the K-major B operand);
 // the tap-shifted one stays channel-minor and reaches wgmma through registers (the register-A form), with the filter taps
@@ -130,21 +131,25 @@ __device__ __forceinline__ void lstm_store(const IgemmArgs& a, long long pix, co
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward / dgrad kernel.  A CTA owns one (BN-column tile, phase, k-split) and walks the 128-pixel tiles
+// forward / dgrad kernel.  A CTA owns one (BN-column tile, phase, k-split) and walks the kRows-pixel tiles
 // m = blockIdx.x, blockIdx.x + gridDim.x, ... (persistent): the TMA ring keeps streaming across tiles, so the loads of
-// tile i+1 overlap the epilogue of tile i.  A ring stage is one 32-channel k-chunk: a 16 KB activation tile (128 rows)
-// and a BN x 128 B weight tile, both 128B-swizzled.  One wgmma group per consumer stays in flight: a stage is released
-// once the group that read it has completed, while the next chunk's MMAs are already queued.
+// tile i+1 overlap the epilogue of tile i.  A ring stage is one 32-channel k-chunk: a kRows x 128 B activation tile and a
+// BN x 128 B weight tile, both 128B-swizzled.  With 128 rows each consumer warpgroup owns one 64-row half of the tile and
+// all BN columns; with 64 rows both read the whole activation tile and each owns BN / 2 of the columns.  One wgmma group
+// per consumer stays in flight: a stage is released once the group that read it has completed, while the next chunk's
+// MMAs are already queued.
 // ------------------------------------------------------------------------------------------------
 constexpr int kFwdThreads = 384;
-template <int BN, bool kLstm, bool kElu = false>
+template <int kRows, int BN, bool kLstm, bool kElu = false>
 __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_constant__ IgemmArgs a) {
+  static_assert(kRows == 128 || (kRows == 64 && BN % 16 == 0 && !kLstm), "64-row tiles split BN into two wgmma N");
+  constexpr int kWN = kRows == 128 ? BN : BN / 2;   // wgmma N of one consumer warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ uint64_t full_bar[kMaxStagesFwd], empty_bar[kMaxStagesFwd];
 
   const int wg = threadIdx.x >> 7;
-  constexpr uint32_t kABytes = 16384u, kStageBytes = kABytes + BN * 128u;
+  constexpr uint32_t kABytes = kRows * 128u, kStageBytes = kABytes + BN * 128u;
   const int num_mtiles = a.tiles_w * a.tiles_h * a.tiles_d * a.tiles_n;
   const int n0 = blockIdx.y * BN;
   const int phase = blockIdx.z / a.splits, split = blockIdx.z % a.splits;
@@ -196,11 +201,14 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
     return;
   }
 
-  // ---- consumers: warpgroup h = wg - 1 owns rows 64 h .. 64 h + 63 of the tile
+  // ---- consumers: warpgroup h = wg - 1 owns rows row0 .. row0 + 63 and columns col0 .. col0 + kWN - 1 of the tile.  A
+  // 64-row offset into the activation tile and a BN / 2-row offset into the weight tile are both whole 1024-byte swizzle
+  // atoms (BN % 16 == 0), so the descriptors start there
   const int h = wg - 1;
+  const int row0 = kRows == 128 ? 64 * h : 0, col0 = kRows == 128 ? 0 : h * kWN;
   const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const uint64_t ad_base = make_wgmma_desc(smem0 + h * 8192u, 16, 1024, kWgmmaSwizzle128B);
-  const uint64_t bd_base = make_wgmma_desc(smem0 + kABytes, 16, 1024, kWgmmaSwizzle128B);
+  const uint64_t ad_base = make_wgmma_desc(smem0 + row0 * 128u, 16, 1024, kWgmmaSwizzle128B);
+  const uint64_t bd_base = make_wgmma_desc(smem0 + kABytes + col0 * 128u, 16, 1024, kWgmmaSwizzle128B);
   constexpr uint32_t kStageAdv = kStageBytes >> 4;
   const int kq_last = a.kc - 1;
   const bool add_bias = (a.bias != nullptr) && (split == 0);
@@ -208,18 +216,18 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
   int lw[2], lh[2], ld[2], ln[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    int row = 64 * h + 16 * wq + (lane >> 2) + 8 * r;
+    int row = row0 + 16 * wq + (lane >> 2) + 8 * r;
     lw[r] = row % a.bw; row /= a.bw;
     lh[r] = row % a.bh; row /= a.bh;
     ld[r] = row % a.bd;
     ln[r] = row / a.bd;
   }
   uint32_t b_off = 0, ph = 0, adv = 0;
-  float acc[BN / 2];
+  float acc[kWN / 2];
 #pragma unroll 1
   for (int mtile = blockIdx.x; mtile < num_mtiles; mtile += gridDim.x) {
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < kWN / 2; ++i) acc[i] = 0.f;
     int kq = it0 % a.kc;
     uint32_t held = 0;     // empty barrier of the stage read by the wgmma group still in flight
 #pragma unroll 1
@@ -231,10 +239,10 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
       const int nk = __all_sync(0xffffffffu, kq == kq_last) ? a.k_tail : 4;
       const uint64_t ad = ad_base + adv, bd = bd_base + adv;
       wgmma_fence();
-      Wgmma<BN>::mma(acc, ad, bd, 1u);
-      if (nk > 1) Wgmma<BN>::mma(acc, ad + 2, bd + 2, 1u);
-      if (nk > 2) Wgmma<BN>::mma(acc, ad + 4, bd + 4, 1u);
-      if (nk > 3) Wgmma<BN>::mma(acc, ad + 6, bd + 6, 1u);
+      Wgmma<kWN>::mma(acc, ad, bd, 1u);
+      if (nk > 1) Wgmma<kWN>::mma(acc, ad + 2, bd + 2, 1u);
+      if (nk > 2) Wgmma<kWN>::mma(acc, ad + 4, bd + 4, 1u);
+      if (nk > 3) Wgmma<kWN>::mma(acc, ad + 6, bd + 6, 1u);
       wgmma_commit();
       // one group stays in flight: the previous chunk's group has completed, so its stage goes back to the producer
       wgmma_wait<1>();
@@ -269,8 +277,8 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
         }
         const long long ooff = on * a.so_n + od * a.so_d + oh * a.so_h + ow * a.so_w;
 #pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-          const int col = n0 + 8 * i + 2 * (lane & 3);
+        for (int i = 0; i < kWN / 8; ++i) {
+          const int col = n0 + col0 + 8 * i + 2 * (lane & 3);
           fwd_store<kElu>(a, ooff, col, acc[4 * i + 2 * r], add_bias);
           fwd_store<kElu>(a, ooff, col + 1, acc[4 * i + 2 * r + 1], add_bias);
         }
@@ -578,20 +586,22 @@ static int build_taps(IgemmArgs& A, const vp_conv_geom* g, int lat[4]) {
   return 0;
 }
 
-// Fills taps / phases / maps for the tap-shifted tensor `sh_t`; the iteration lattice has dims `lat`.
-static int build_geometry(IgemmArgs& A, const vp_conv_geom* g, const vp_tensor* sh_t, int rows_per_tile,
-                          const int lat_in[4] /*w,h,d,n*/) {
-  int lat[4] = {lat_in[0], lat_in[1], lat_in[2], lat_in[3]};
-  if (build_taps(A, g, lat)) return -1;
-  // box shape: product == rows_per_tile, powers of two, w fastest
-  int rem = rows_per_tile;
-  A.bw = std::min(floor_pow2(lat[0]), rem); rem /= A.bw;
-  A.bh = std::min(floor_pow2(lat[1]), rem); rem /= A.bh;
-  A.bd = std::min(floor_pow2(lat[2]), rem); rem /= A.bd;
-  A.bn = rem;
-  A.tiles_w = ceil_div(lat[0], A.bw); A.tiles_h = ceil_div(lat[1], A.bh);
-  A.tiles_d = ceil_div(lat[2], A.bd); A.tiles_n = ceil_div(lat[3], A.bn);
-  const int box[4] = {A.bw, A.bh, A.bd, A.bn};
+// Box of a `rows`-pixel tile over the iteration lattice `lat` (w,h,d,n): powers of two, w fastest, product == rows.
+// Returns the number of tiles.
+static int tile_box(const int lat[4], int rows, int box[4], int tiles[4]) {
+  int rem = rows, m_tiles = 1;
+  for (int i = 0; i < 3; ++i) { box[i] = std::min(floor_pow2(lat[i]), rem); rem /= box[i]; }
+  box[3] = rem;
+  for (int i = 0; i < 4; ++i) { tiles[i] = ceil_div(lat[i], box[i]); m_tiles *= tiles[i]; }
+  return m_tiles;
+}
+
+// Tile box and one activation map per stride parity (one for a transposed conv) of the tap-shifted tensor `sh_t`.
+static int build_maps(IgemmArgs& A, const vp_conv_geom* g, const vp_tensor* sh_t, int rows_per_tile, const int lat[4]) {
+  int box[4], tiles[4];
+  tile_box(lat, rows_per_tile, box, tiles);
+  A.bw = box[0]; A.bh = box[1]; A.bd = box[2]; A.bn = box[3];
+  A.tiles_w = tiles[0]; A.tiles_h = tiles[1]; A.tiles_d = tiles[2]; A.tiles_n = tiles[3];
   if (!g->transposed) {
     for (int qd = 0; qd < g->sd; ++qd)
       for (int qh = 0; qh < g->sh; ++qh)
@@ -606,7 +616,6 @@ static int build_geometry(IgemmArgs& A, const vp_conv_geom* g, const vp_tensor* 
   return 0;
 }
 
-
 }  // namespace vp
 
 using namespace vp;
@@ -620,6 +629,69 @@ struct LstmCell {
   int num_h;
   float forget_bias;
 };
+
+typedef void (*FwdKernel)(const IgemmArgs);
+struct FwdForm {
+  int rows, bn;        // pixels x GEMM columns of a tile
+  float chunk_us;      // time of one 32-channel k-chunk of one CTA with every SM busy
+  FwdKernel kernel[2]; // plain, ELU
+};
+// Forms of igemm_fwd_kernel.  The first is the ConvLSTM cell's and is not a candidate of pick_fwd_form.  The others are
+// the forms pick_fwd_form chooses for the calls of the cfg2 training step; BN = 80 and 144 match the n_pad of its 2F + nz
+// input widths (nz = 8) without padded columns.  A last column tile that reaches past n_pad multiplies rows of the next
+// tap's weights (or TMA zero fill) into columns that are never stored.  chunk_us is the median over the 55 distinct
+// forward / dgrad calls of the cfg2 step of (call time) / (waves x k-chunks per tile), each call timed in every form (CUDA
+// graphs of 10 calls, median of 5 replays; NVIDIA H100 80GB HBM3, 700 W power limit, 1980 MHz max SM clock).  With these
+// costs the rule's picks take those calls from 48.5 to 39.9 ms per step, against 39.8 ms for the fastest form of each.
+static const FwdForm kFwdForms[] = {
+    {128, 128, 0.f, {igemm_fwd_kernel<128, 128, true>, nullptr}},
+    {128, 32, 0.448f, {igemm_fwd_kernel<128, 32, false>, igemm_fwd_kernel<128, 32, false, true>}},
+    {128, 64, 0.565f, {igemm_fwd_kernel<128, 64, false>, igemm_fwd_kernel<128, 64, false, true>}},
+    {128, 80, 0.634f, {igemm_fwd_kernel<128, 80, false>, igemm_fwd_kernel<128, 80, false, true>}},
+    {128, 128, 0.736f, {igemm_fwd_kernel<128, 128, false>, igemm_fwd_kernel<128, 128, false, true>}},
+    {64, 32, 0.371f, {igemm_fwd_kernel<64, 32, false>, igemm_fwd_kernel<64, 32, false, true>}},
+    {64, 64, 0.429f, {igemm_fwd_kernel<64, 64, false>, igemm_fwd_kernel<64, 64, false, true>}},
+    {64, 80, 0.455f, {igemm_fwd_kernel<64, 80, false>, igemm_fwd_kernel<64, 80, false, true>}},
+    {64, 128, 0.548f, {igemm_fwd_kernel<64, 128, false>, igemm_fwd_kernel<64, 128, false, true>}},
+    {64, 144, 0.577f, {igemm_fwd_kernel<64, 144, false>, igemm_fwd_kernel<64, 144, false, true>}},
+};
+constexpr int kNumFwdForms = static_cast<int>(sizeof(kFwdForms) / sizeof(kFwdForms[0]));
+
+// The form of a forward / dgrad call, from its shape alone: the one with the least estimated time, waves of CTAs x
+// k-chunks per tile x the form's cost per chunk (ties: the earlier form).  `lat` is the iteration lattice (w,h,d,n);
+// `z` = phases x k-splits, the grid's third dimension.
+static int pick_fwd_form(const int lat[4], int n_pad, int z, int chunks, int sms) {
+  int best = 1;
+  double best_t = 1e30;
+  for (int f = 1; f < kNumFwdForms; ++f) {
+    int box[4], tiles[4];
+    const int m_tiles = tile_box(lat, kFwdForms[f].rows, box, tiles);
+    const int other = ceil_div(n_pad, kFwdForms[f].bn) * z;
+    const int gx = std::min(m_tiles, std::max(1, sms / other));
+    const double waves = static_cast<double>(ceil_div(m_tiles, gx)) * ceil_div(gx * other, sms);
+    const double t = waves * chunks * kFwdForms[f].chunk_us;
+    if (t < best_t) { best_t = t; best = f; }
+  }
+  return best;
+}
+
+// Taps, phases and k-splits of a forward / dgrad call into A, `lat` (w,h,d,n: the output) turned into the iteration
+// lattice; returns the index of the call's form in kFwdForms, -1 on error.
+static int plan_fwd(IgemmArgs& A, const vp_conv_geom* g, int lat[4], int n_pad, int kc, int split_k, int sms) {
+  if (build_taps(A, g, lat)) return -1;
+  A.kc = kc; A.n_pad = n_pad;
+  int max_iters = 0, min_iters = 1 << 30;
+  for (int p = 0; p < A.num_phases; ++p) {
+    const int iters = (A.phase_begin[p + 1] - A.phase_begin[p]) * kc;
+    max_iters = std::max(max_iters, iters);
+    min_iters = std::min(min_iters, iters);
+  }
+  if (min_iters < 1) return set_error("vp_conv_igemm: a phase has no taps");
+  // split_k == 0 (automatic) runs unsplit: split partial sums are added with atomics, whose order (and so the fp32 result)
+  // would change from run to run
+  A.splits = std::max(1, std::min(std::max(split_k, 1), min_iters));
+  return pick_fwd_form(lat, n_pad, A.num_phases * A.splits, ceil_div(max_iters, A.splits), sms);
+}
 
 static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,
                            const vp_tensor* out, const float* bias, int act, float alpha, int split_k, int accumulate,
@@ -640,35 +712,21 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
     return set_error("vp_conv_igemm: accumulate = 2 needs split_k <= 1 (got split_k = %d)", split_k);
   static thread_local IgemmArgs A;  // large POD; per-thread host-side scratch (ctypes releases the GIL during calls)
   std::memset(&A, 0, sizeof(A));
-  const int lat[4] = {out->w, out->h, out->d, out->n};
-  if (build_geometry(A, g, in, 128, lat)) return -1;
-  A.kc = kc; A.n_pad = n_pad;
+  int lat[4] = {out->w, out->h, out->d, out->n};
+  const int sms = device_sms();
+  const int f = plan_fwd(A, g, lat, n_pad, kc, split_k, sms);
+  if (f < 0) return -1;
   A.k_tail = std::min(4, std::max(1, ceil_div(in->c - (kc - 1) * 32, 8)));
-  // N tiling: the wgmma N of the tile (32, 64 or 128) whose tiles cover n_pad with the fewest padded columns (ties: the
-  // wider tile, which reads the activations fewer times).  A last tile that reaches past n_pad multiplies rows of the next
-  // tap's weights (or TMA zero fill) into columns that are never stored.
-  {
-    int best = 1 << 30;
-    for (int bn : {128, 64, 32}) {
-      const int cols = ceil_div(n_pad, bn) * bn;
-      if (cols < best) { best = cols; A.bn_tile = bn; }
-    }
-  }
-  if (cell) {     // a 128-column tile holds all four gates of 32 cell channels
-    A.bn_tile = 128;
+  // a 128 x 128 tile holds all four gates of 32 cell channels
+  const FwdForm& form = kFwdForms[cell ? 0 : f];
+  A.bn_tile = form.bn;
+  if (build_maps(A, g, in, form.rows, lat)) return -1;
+  if (cell) {
     A.lstm_f = out->c / 4;
     A.c_prev = cell->c_prev; A.c_new = cell->c_new; A.num_h = cell->num_h; A.forget_bias = cell->forget_bias;
     for (int i = 0; i < cell->num_h; ++i) { A.h_dst[i] = cell->h_dst[i]; A.h_cs[i] = cell->h_cs[i]; }
   }
   const int n_tiles = ceil_div(n_pad, A.bn_tile);
-  int min_iters = 1 << 30;
-  for (int p = 0; p < A.num_phases; ++p) min_iters = std::min(min_iters, (A.phase_begin[p + 1] - A.phase_begin[p]) * kc);
-  if (min_iters < 1) return set_error("vp_conv_igemm: a phase has no taps");
-  const int sms = device_sms();
-  // split_k == 0 (automatic) runs unsplit: split partial sums are added with atomics, whose order (and so the fp32 result)
-  // would change from run to run
-  if (split_k <= 0) split_k = 1;
-  A.splits = std::max(1, std::min(split_k, min_iters));
   A.aux_y = aux_y; A.aux_add = aux_add; A.aux_act = aux_act;
   A.out = out->ptr;
   A.so_w = out->cstride; A.so_h = A.so_w * out->w; A.so_d = A.so_h * out->h; A.so_n = A.so_d * out->d;
@@ -691,23 +749,20 @@ static int conv_igemm_impl(const vp_tensor* in, const vp_conv_geom* g, const flo
     if (r != CUDA_SUCCESS) return set_error("cuTensorMapEncodeTiled(weights) failed with %d", static_cast<int>(r));
   }
   // ring depth: as many one-chunk stages as fit next to the static shared memory
-  const size_t stage_bytes = 16384 + static_cast<size_t>(A.bn_tile) * 128;
+  const size_t stage_bytes = static_cast<size_t>(form.rows + A.bn_tile) * 128;
   const size_t smem_max = 227 * 1024 - 2048;
   A.stages = static_cast<int>(std::min<size_t>(kMaxStagesFwd, (smem_max - 1024) / stage_bytes));
   const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
-  typedef void (*FwdKernel)(const IgemmArgs);
-  static const FwdKernel kernels[7] = {igemm_fwd_kernel<32, false>, igemm_fwd_kernel<64, false>, igemm_fwd_kernel<128, false>,
-                                       igemm_fwd_kernel<128, true>, igemm_fwd_kernel<32, false, true>,
-                                       igemm_fwd_kernel<64, false, true>, igemm_fwd_kernel<128, false, true>};
   static bool attr_set = false;
   if (!attr_set) {
-    for (FwdKernel k : kernels)
-      if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
-        return set_error("cudaFuncSetAttribute(igemm_fwd_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
+    for (const FwdForm& fm : kFwdForms)
+      for (FwdKernel k : fm.kernel)
+        if (k && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
+          return set_error("cudaFuncSetAttribute(igemm_fwd_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
     attr_set = true;
   }
   const bool elu = act == VP_ACT_ELU || (aux_y && aux_act == VP_ACT_ELU);
-  const FwdKernel kernel = kernels[cell ? 3 : (A.bn_tile == 32 ? 0 : A.bn_tile == 64 ? 1 : 2) + (elu ? 4 : 0)];
+  const FwdKernel kernel = form.kernel[elu ? 1 : 0];
   // persistent over the pixel tiles: one CTA per SM in total; each CTA strides through the M tiles
   const int m_tiles = A.tiles_w * A.tiles_h * A.tiles_d * A.tiles_n;
   const int other = n_tiles * A.num_phases * A.splits;
@@ -721,6 +776,24 @@ extern "C" int vp_conv_igemm(const vp_tensor* in, const vp_conv_geom* g, const f
                              const vp_tensor* out, const float* bias, int act, float alpha, int split_k,
                              int accumulate, vp_stream_t stream) {
   return conv_igemm_impl(in, g, wpacked, n_pad, kc, out, bias, act, alpha, split_k, accumulate, nullptr, nullptr, 0, stream);
+}
+
+extern "C" int vp_conv_igemm_form(const vp_conv_geom* g, const int out_ndhw[4], int n_pad, int kc, int split_k, int sms,
+                                  int* rows, int* bn) {
+  if (!g || !out_ndhw || !rows || !bn || sms < 1 || kc < 1) return set_error("vp_conv_igemm_form: bad argument");
+  static thread_local IgemmArgs A;
+  std::memset(&A, 0, sizeof(A));
+  int lat[4] = {out_ndhw[3], out_ndhw[2], out_ndhw[1], out_ndhw[0]};
+  const int f = plan_fwd(A, g, lat, n_pad, kc, split_k, sms);
+  if (f < 0) return -1;
+  *rows = kFwdForms[f].rows;
+  *bn = kFwdForms[f].bn;
+  return 0;
+}
+
+extern "C" int vp_conv_igemm_forms(int* rows, int* bn, int cap) {
+  for (int f = 1; f < kNumFwdForms && f <= cap; ++f) { rows[f - 1] = kFwdForms[f].rows; bn[f - 1] = kFwdForms[f].bn; }
+  return kNumFwdForms - 1;
 }
 
 extern "C" int vp_conv_igemm_actgrad(const vp_tensor* in, const vp_conv_geom* g, const float* wpacked, int n_pad, int kc,

@@ -150,6 +150,22 @@ def conv_igemm(x_view, g, wpacked, n_pad, kc, out_view, bias=None, act=ACT_NONE,
                                                 act, C.c_float(alpha), split_k, int(accumulate), stream_ptr())))
 
 
+def conv_igemm_form(g, out_ndhw, n_pad, kc, sms, split_k=1):
+    """(pixel rows, GEMM columns) of the tile vp_conv_igemm / vp_conv_igemm_actgrad launch for this call shape on `sms`
+    SMs; out_ndhw = the output's (n, d, h, w).  Needs no device."""
+    rows, bn = C.c_int(), C.c_int()
+    check(lib().vp_conv_igemm_form(C.byref(g), (C.c_int * 4)(*out_ndhw), n_pad, kc, split_k, sms, C.byref(rows), C.byref(bn)))
+    return rows.value, bn.value
+
+
+def conv_igemm_forms():
+    """Every (pixel rows, GEMM columns) tile that conv_igemm_form can return."""
+    n = lib().vp_conv_igemm_forms(None, None, 0)
+    rows, bn = (C.c_int * n)(), (C.c_int * n)()
+    lib().vp_conv_igemm_forms(rows, bn, n)
+    return list(zip(rows, bn))
+
+
 def conv_igemm_actgrad(x_view, g, wpacked, n_pad, kc, out_view, act_output_addr, addend_addr, act, alpha=0.0, accumulate=0):
     if 'igemm' in _SKIP:
         return

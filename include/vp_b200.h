@@ -189,6 +189,15 @@ int vp_dense_fwd(const float* x, int x_stride, const float* w, const float* bias
 /* tf.nn.rnn_cell.LSTMCell elementwise part (savp_model.py:354-362); gates [b][4*units] (i,j,f,o). */
 int vp_lstm_cell_fwd(const float* gates, const float* c_prev, float* c_new, float* h_new, int b, int units,
                      float forget_bias, vp_stream_t stream);
+/* tf.contrib.rnn.GRUCell elementwise parts (TF >= 1.9, savp_model.py:354-362), around its `gates` and `candidate` dense
+ * layers; gates [b][2*units] pre-activations (r, u), h_prev [b][units].
+ *   stage 0: rh[b][rh_cstride] = sigmoid(r) * h_prev (the h lanes of the candidate layer's input [z, r*h]);
+ *   stage 1: h_new = u * h_prev + (1 - u) * tanh(cand), cand [b][units] the candidate pre-activation. */
+int vp_gru_cell_fwd(int stage, const float* gates, const float* h_prev, const float* cand, float* rh, int rh_cstride,
+                    float* h_new, int b, int units, vp_stream_t stream);
+/* y[r][0..c) = act(x[r][0..c)), any VP_ACT_* (the forward twin of vp_act_bwd). */
+int vp_act_fwd(const float* x, int x_cstride, float* y, int y_cstride, long long rows, int c, int act, float alpha,
+               vp_stream_t stream);
 /* savp_model.py:49,712: lss <- clip(lss,-10,10); z = mu + sqrt(exp(lss))*eps. */
 int vp_sample_z(const float* mu, float* log_sigma_sq, const float* eps, float* z, int total, vp_stream_t stream);
 /* savp_model.py:551-559: +identity kernel, relu(.-1e-12)+1e-12, normalise over the kh*kw taps.
@@ -279,6 +288,13 @@ int vp_dense_bwd(const float* x, int x_stride, const float* w, const float* inv_
                  vp_stream_t stream);
 int vp_lstm_cell_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh, const float* dc_next,
                      float* dgates, float* dc_prev, int b, int units, float forget_bias, vp_stream_t stream);
+/* vp_gru_cell_fwd backward, around the two dense backwards:
+ *   stage 0 (dh = dL/dh_new): dcand = dh (1-u)(1-c^2) with c = tanh(cand), dgates[.., units + i] = dh (h_prev - c) u(1-u),
+ *            dh_prev = dh u;
+ *   stage 1 (drh [b][drh_cstride] = dL/d(r*h), the candidate dense backward's h lanes): dgates[.., i] = drh h_prev r(1-r),
+ *            dh_prev += drh r. */
+int vp_gru_cell_bwd(int stage, const float* gates, const float* h_prev, const float* cand, const float* dh, const float* drh,
+                    int drh_cstride, float* dgates, float* dcand, float* dh_prev, int b, int units, vp_stream_t stream);
 /* out[n*out_stride + c] += scale * sum_p x[n][p][c] */
 int vp_colsum(const float* x, int x_cstride, float* out, int out_stride, int n, long long positions, int c, float scale,
               vp_stream_t stream);

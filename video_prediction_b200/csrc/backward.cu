@@ -603,6 +603,31 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ gates, const floa
   dc_prev[idx] = dc * sf;
 }
 
+// dense GRU cell backward (gru_cell_fwd_kernel), around the two dense backwards:
+// stage 0, from dh of h' = u h + (1 - u) c, c = tanh(cand): dcand, the u lanes of dgates, dh_prev = dh u;
+// stage 1, from drh of the candidate input's rh = r h lanes: the r lanes of dgates, dh_prev += drh r.
+__global__ void gru_cell_bwd_kernel(int stage, const float* __restrict__ gates, const float* __restrict__ h_prev,
+                                    const float* __restrict__ cand, const float* __restrict__ dh, const float* __restrict__ drh,
+                                    int drhs, float* __restrict__ dgates, float* __restrict__ dcand, float* __restrict__ dh_prev,
+                                    int B, int U) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * U) return;
+  const int b = idx / U, u = idx % U;
+  const float* g = gates + static_cast<long long>(b) * 2 * U;
+  float* dg = dgates + static_cast<long long>(b) * 2 * U;
+  const float h = h_prev[idx];
+  if (stage == 0) {
+    const float ug = sigm(g[U + u]), c = tanhf(cand[idx]), d = dh[idx];
+    dcand[idx] = d * (1.f - ug) * (1.f - c * c);
+    dg[U + u] = d * (h - c) * ug * (1.f - ug);
+    dh_prev[idx] = d * ug;
+    return;
+  }
+  const float r = sigm(g[u]), d = drh[static_cast<long long>(b) * drhs + u];
+  dg[u] = d * h * r * (1.f - r);
+  dh_prev[idx] += d * r;
+}
+
 // norm-free ConvLSTM cell backward (vp_conv_lstm_fwd): one thread per (row, cell channel), dh summed in source order
 __global__ void lstm_plain_bwd_kernel(const float* __restrict__ z, const float* __restrict__ c_prev,
                                       const float* __restrict__ c_new, SrcList dh, const float* __restrict__ dc_next,
@@ -1073,6 +1098,18 @@ extern "C" int vp_lstm_cell_bwd(const float* gates, const float* c_prev, const f
   lstm_cell_bwd_kernel<<<grid_for(static_cast<long long>(b) * units, 128), 128, 0, as_stream(stream)>>>(
       gates, c_prev, c_new, dh, dc_next, dgates, dc_prev, b, units, forget_bias);
   return check_launch("lstm_cell_bwd_kernel");
+}
+
+extern "C" int vp_gru_cell_bwd(int stage, const float* gates, const float* h_prev, const float* cand, const float* dh,
+                               const float* drh, int drh_cstride, float* dgates, float* dcand, float* dh_prev, int b, int units,
+                               vp_stream_t stream) {
+  if (stage != 0 && stage != 1) return set_error("vp_gru_cell_bwd: stage must be 0 or 1, got %d", stage);
+  if (!gates || !h_prev || !dgates || !dh_prev || (stage == 0 ? (!cand || !dh || !dcand) : !drh))
+    return set_error("vp_gru_cell_bwd: null pointer");
+  if (b < 1 || units < 1 || (stage == 1 && drh_cstride < units)) return set_error("vp_gru_cell_bwd: bad b / units / drh stride");
+  gru_cell_bwd_kernel<<<grid_for(static_cast<long long>(b) * units, 128), 128, 0, as_stream(stream)>>>(
+      stage, gates, h_prev, cand, dh, drh, drh_cstride, dgates, dcand, dh_prev, b, units);
+  return check_launch("gru_cell_bwd_kernel");
 }
 
 extern "C" int vp_colsum(const float* x, int x_cstride, float* out, int out_stride, int n, long long positions, int c,

@@ -354,6 +354,34 @@ __global__ void lstm_cell_fwd_kernel(const float* __restrict__ gates, const floa
   h_new[idx] = tanhf(c) * sigmoidf_(g[3 * U + u]);
 }
 
+// dense GRU cell on z (tf.contrib.rnn.GRUCell, TF >= 1.9; savp_model.py:354-362): gates [B,2U] pre-activations (r, u).
+// stage 0: rh = sigmoid(r) * h_prev, the h lanes of the candidate layer's input; stage 1: h' = u h + (1 - u) tanh(cand).
+__global__ void gru_cell_fwd_kernel(int stage, const float* __restrict__ gates, const float* __restrict__ h_prev,
+                                    const float* __restrict__ cand, float* __restrict__ rh, int rhs, float* __restrict__ h_new,
+                                    int B, int U) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * U) return;
+  const int b = idx / U, u = idx % U;
+  const float* g = gates + static_cast<long long>(b) * 2 * U;
+  if (stage == 0) {
+    rh[static_cast<long long>(b) * rhs + u] = sigmoidf_(g[u]) * h_prev[idx];
+    return;
+  }
+  const float ug = sigmoidf_(g[U + u]);
+  h_new[idx] = ug * h_prev[idx] + (1.f - ug) * tanhf(cand[idx]);
+}
+
+// y = act(x) on channel slices (the forward twin of act_bwd_from_output_kernel)
+template <bool kElu>
+__global__ void act_fwd_kernel(const float* __restrict__ x, int xs, float* __restrict__ y, int ys, long long total, int C, int act,
+                               float alpha) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int c = static_cast<int>(idx % C);
+  const long long r = idx / C;
+  y[r * ys + c] = act_fwd<kElu>(x[r * xs + c], act, alpha);
+}
+
 // z = mu + sqrt(exp(clip(lss,-10,10))) * eps  (savp_model.py:49, 712); also writes the clipped lss
 __global__ void sample_z_kernel(const float* __restrict__ mu, float* __restrict__ lss, const float* __restrict__ eps,
                                 float* __restrict__ z, int total) {
@@ -591,6 +619,27 @@ extern "C" int vp_lstm_cell_fwd(const float* gates, const float* c_prev, float* 
   lstm_cell_fwd_kernel<<<grid_for(static_cast<long long>(b) * units, 128), 128, 0, as_stream(stream)>>>(
       gates, c_prev, c_new, h_new, b, units, forget_bias);
   return check_launch("lstm_cell_fwd_kernel");
+}
+
+extern "C" int vp_gru_cell_fwd(int stage, const float* gates, const float* h_prev, const float* cand, float* rh, int rh_cstride,
+                               float* h_new, int b, int units, vp_stream_t stream) {
+  if (stage != 0 && stage != 1) return set_error("vp_gru_cell_fwd: stage must be 0 or 1, got %d", stage);
+  if (!gates || !h_prev || (stage == 0 ? !rh : (!cand || !h_new))) return set_error("vp_gru_cell_fwd: null pointer");
+  if (b < 1 || units < 1 || (stage == 0 && rh_cstride < units)) return set_error("vp_gru_cell_fwd: bad b / units / rh stride");
+  gru_cell_fwd_kernel<<<grid_for(static_cast<long long>(b) * units, 128), 128, 0, as_stream(stream)>>>(
+      stage, gates, h_prev, cand, rh, rh_cstride, h_new, b, units);
+  return check_launch("gru_cell_fwd_kernel");
+}
+
+extern "C" int vp_act_fwd(const float* x, int x_cstride, float* y, int y_cstride, long long rows, int c, int act, float alpha,
+                          vp_stream_t stream) {
+  if (check_act(act, "vp_act_fwd")) return -1;
+  if (!x || !y || rows < 0 || c < 1 || x_cstride < c || y_cstride < c) return set_error("vp_act_fwd: bad pointer / shape");
+  const long long total = rows * c;
+  if (total == 0) return 0;
+  (act == VP_ACT_ELU ? act_fwd_kernel<true> : act_fwd_kernel<false>)<<<grid_for(total, 256), 256, 0, as_stream(stream)>>>(
+      x, x_cstride, y, y_cstride, total, c, act, alpha);
+  return check_launch("act_fwd_kernel");
 }
 
 extern "C" int vp_sample_z(const float* mu, float* log_sigma_sq, const float* eps, float* z, int total,

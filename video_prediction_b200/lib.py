@@ -367,6 +367,15 @@ def lstm_cell_fwd(gates, c_prev, c_new, h_new, b, units, forget_bias=1.0):
     check(lib().vp_lstm_cell_fwd(ptr(gates), ptr(c_prev), ptr(c_new), ptr(h_new), b, units, _f(forget_bias), stream_ptr()))
 
 
+def gru_cell_fwd(stage, gates, h_prev, cand, rh_addr, rh_cs, h_new, b, units):
+    check(lib().vp_gru_cell_fwd(stage, ptr(gates), ptr(h_prev), ptr(cand), addr(rh_addr or 0), rh_cs, ptr(h_new), b, units,
+                                stream_ptr()))
+
+
+def act_fwd(x_addr, x_cs, y_addr, y_cs, rows, c, act, alpha=0.0):
+    check(lib().vp_act_fwd(addr(x_addr), x_cs, addr(y_addr), y_cs, C.c_longlong(rows), c, act, _f(alpha), stream_ptr()))
+
+
 def sample_z(mu, lss, eps, z, total):
     check(lib().vp_sample_z(ptr(mu), ptr(lss), ptr(eps), ptr(z), total, stream_ptr()))
 
@@ -531,6 +540,11 @@ def dense_bwd(x, x_stride, w, dy, dy_stride, b, k, j, dx=None, dx_stride=0, dx_a
 def lstm_cell_bwd(gates, c_prev, c_new, dh, dc_next, dgates, dc_prev, b, units, forget_bias=1.0):
     check(lib().vp_lstm_cell_bwd(ptr(gates), ptr(c_prev), ptr(c_new), ptr(dh), ptr(dc_next), ptr(dgates), ptr(dc_prev), b, units,
                                  _f(forget_bias), stream_ptr()))
+
+
+def gru_cell_bwd(stage, gates, h_prev, cand, dh, drh_addr, drh_cs, dgates, dcand, dh_prev, b, units):
+    check(lib().vp_gru_cell_bwd(stage, ptr(gates), ptr(h_prev), ptr(cand), ptr(dh), addr(drh_addr or 0), drh_cs, ptr(dgates),
+                                ptr(dcand), ptr(dh_prev), b, units, stream_ptr()))
 
 
 def colsum(x_addr, x_cs, out, n, positions, c, scale=1.0, out_stride=None):

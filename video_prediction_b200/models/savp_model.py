@@ -263,13 +263,14 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 raise ValueError('Invalid %s layer %s' % (key, getattr(hp, key + '_layer')))
         unsupported = []
         for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('rnn', 'lstm'), ('use_e_rnn', False), ('learn_prior', False),
-                          ('learn_initial_state', False), ('ablation_rnn', False),
-                          ('use_rnn_z', True), ('joint_gan_optimization', False), ('use_same_discriminator', False)):
+                          ('conv_rnn', 'lstm'), ('use_e_rnn', False), ('learn_prior', False),
+                          ('joint_gan_optimization', False), ('use_same_discriminator', False)):
             # (`repeat` is accepted with any value: train.py sets it to the dataset's time_shift (train.py:160) and no model
             #  code of the reference reads it, base_model.py:90-95)
             if getattr(hp, key) != want:
                 unsupported.append('%s=%r' % (key, getattr(hp, key)))
+        if hp.rnn not in ('lstm', 'gru'):      # the z cell (savp_model.py:354-362)
+            unsupported.append('rnn=%r' % (hp.rnn,))
         # the normaliser of every convolution outside the ConvLSTM cells (savp_model.py:394, ops.py:1062-1073): instance,
         # layer or none; 'batch' would need moving averages and a train / test switch
         if hp.norm_layer not in ('instance', 'layer', 'none'):
@@ -278,7 +279,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         # instance norm on the cell's output
         if hp.conv_rnn_norm_layer not in ('instance', 'none'):
             unsupported.append('conv_rnn_norm_layer=%r' % (hp.conv_rnn_norm_layer,))
-        elif hp.ablation_conv_rnn_norm and hp.conv_rnn_norm_layer == 'none':
+        elif hp.ablation_conv_rnn_norm and hp.conv_rnn_norm_layer == 'none' and not hp.ablation_rnn:
             raise ValueError('ablation_conv_rnn_norm=True needs a conv_rnn_norm_layer to apply to the cell output, got '
                              "'none'")   # the reference calls None(h) (savp_model.py:380-383)
         if hp.transformation not in ('cdna', 'flow'):
@@ -328,6 +329,15 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         """True: the reference's default ConvLSTM, with instance norms inside the cell.  False: the norm-free cell
         (conv_rnn_norm_layer='none', or the ablation_conv_rnn_norm form), whose gate math runs in the engine's epilogue."""
         return self.hparams.conv_rnn_norm_layer == 'instance' and not self.hparams.ablation_conv_rnn_norm
+
+    @property
+    def z_cell(self):
+        """The cell rnn_z comes from (savp_model.py:424-432): 'lstm' / 'gru' (`rnn`), 'fc' (ablation_rnn: tanh(dense(z))), or
+        None -- no z, or use_rnn_z=False, where the zs themselves go into the tile-concat vector."""
+        hp = self.hparams
+        if not hp.nz or not hp.use_rnn_z:
+            return None
+        return 'fc' if hp.ablation_rnn else hp.rnn
 
     @property
     def norm_scope(self):
@@ -397,9 +407,18 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 specs['%s/%s/dense/kernel' % (sc, nm)] = ((cin, hp.nz), 'kernel')
                 specs['%s/%s/dense/bias' % (sc, nm)] = ((hp.nz,), 'zeros')
         sc = 'generator/rnn/savp_cell'
-        if hp.nz:
-            specs[sc + '/lstm_z/basic_lstm_cell/kernel'] = ((2 * hp.nz, 4 * hp.nz), 'kernel')
-            specs[sc + '/lstm_z/basic_lstm_cell/bias'] = ((4 * hp.nz,), 'zeros')
+        nz = hp.nz
+        if self.z_cell == 'lstm':
+            specs[sc + '/lstm_z/basic_lstm_cell/kernel'] = ((2 * nz, 4 * nz), 'kernel')
+            specs[sc + '/lstm_z/basic_lstm_cell/bias'] = ((4 * nz,), 'zeros')
+        elif self.z_cell == 'gru':     # GRUCell (TF >= 1.9): the gate bias starts at 1
+            specs[sc + '/gru_z/gru_cell/gates/kernel'] = ((2 * nz, 2 * nz), 'kernel')
+            specs[sc + '/gru_z/gru_cell/gates/bias'] = ((2 * nz,), 'ones')
+            specs[sc + '/gru_z/gru_cell/candidate/kernel'] = ((2 * nz, nz), 'kernel')
+            specs[sc + '/gru_z/gru_cell/candidate/bias'] = ((nz,), 'zeros')
+        elif self.z_cell == 'fc':
+            specs[sc + '/fc_z/dense/kernel'] = ((nz, nz), 'kernel')
+            specs[sc + '/fc_z/dense/bias'] = ((nz,), 'zeros')
 
         def norm(name, c):
             specs[name + '/gamma'] = ((c,), 'ones')
@@ -410,6 +429,11 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 norm('%s/%s' % (site, self.norm_scope), c)
 
         def lstm(i, cin, oc):
+            if hp.ablation_rnn:     # conv 5x5 + norm_layer + activation_layer, no state (savp_model.py:472-475)
+                specs['%s/conv_h%d/conv2d/kernel' % (sc, i)] = ((5, 5, cin + Zc, oc), 'kernel')
+                specs['%s/conv_h%d/conv2d/bias' % (sc, i)] = ((oc,), 'zeros')
+                site_norm('%s/conv_h%d' % (sc, i), oc)
+                return
             b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, i)
             specs[b + '/kernel'] = ((5, 5, cin + Zc + oc, 4 * oc), 'kernel')
             if self.cell_norm:
@@ -471,7 +495,29 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if self.Sd:       # savp_model.py:655-658: the next robot state from [actions | state]
             specs[sc + '/state_pred/dense/kernel'] = ((A + self.Sd, self.Sd), 'kernel')
             specs[sc + '/state_pred/dense/bias'] = ((self.Sd,), 'zeros')
+        for name, shape, _, _ in self._initial_state_specs():
+            specs[name] = (shape, 'zeros')
         return specs
+
+    def _initial_state_specs(self):
+        """learn_initial_state (savp_model.py:263-307, 344-348): [(name, shape, state, li)] in the order of nest.flatten of
+        {'conv_rnn_states': [LSTMStateTuple(c, h) per ConvLSTM, in layer order], 'rnn_z_state': (c, h) of lstm_z or h of
+        gru_z} -- dict keys sorted, so the ConvLSTMs first.  `state` names the buffer the variable initialises: 'c' / 'h' of
+        generator layer li, 'zc' / 'zh'.  No ConvLSTM entries under ablation_rnn, no z entry without a z RNN."""
+        hp = self.hparams
+        if not hp.learn_initial_state:
+            return []
+        leaves = []
+        if not hp.ablation_rnn:
+            hh, ww = self.H, self.W
+            for li, (oc, use) in enumerate(self.enc_specs + self.dec_specs):
+                hh, ww = (hh // 2, ww // 2) if li < len(self.enc_specs) else (hh * 2, ww * 2)
+                if use:
+                    leaves += [((hh, ww, oc), 'c', li), ((hh, ww, oc), 'h', li)]
+        if self.z_cell in ('lstm', 'gru'):
+            leaves += [((hp.nz,), 'zc', -1)] if self.z_cell == 'lstm' else []
+            leaves.append(((hp.nz,), 'zh', -1))
+        return [('generator/initial_state_%d/initial_state' % k, shape, what, li) for k, (shape, what, li) in enumerate(leaves)]
 
     # ------------------------------------------------------------------ build
     def build_graph(self, inputs):
@@ -842,7 +888,19 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             self.convs.append(d['conv'])
             Bf['pre%d' % li] = self._z(S, NB, hh, ww, oc)
             Bf['nst%d' % li] = self._norm_stats(S, NB, oc)
-            if use:
+            if use and hp.ablation_rnn:
+                # the stateless conv_h{li} site on (h{li} | z): conv -> rpre -> norm + activation -> out
+                d['rin_spec'] = ConcatSpec([('x', oc)] + zseg)
+                Bf['rin%d' % li] = self._z(S, NB, hh, ww, d['rin_spec'].cstride)
+                s = '%s/conv_h%d' % (sc, li)
+                d['rconv'] = ConvLayer(self, s + '/conv2d/kernel', s + '/conv2d/bias', (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
+                                       (0, 2, 2), False, d['rin_spec'], oc)
+                d['rname'] = s
+                self.convs.append(d['rconv'])
+                Bf['rpre%d' % li] = self._z(S, NB, hh, ww, oc)
+                Bf['rnst%d' % li] = self._norm_stats(S, NB, oc)
+                Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
+            elif use:
                 d['rin_spec'] = ConcatSpec([('x', oc)] + zseg + [('h', oc)])
                 Bf['rin%d' % li] = self._z(S + 1, NB, hh, ww, d['rin_spec'].cstride)
                 b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, li)
@@ -853,6 +911,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 self.convs.append(d['rconv'])
                 Bf['gpre%d' % li] = self._z(S, NB, hh, ww, 4 * oc)
                 Bf['c%d' % li] = self._z(S + 1, NB, hh, ww, oc)      # c[t] = state entering step t
+                if hp.learn_initial_state:
+                    Bf['h0_%d' % li] = self._z(NB, hh, ww, oc)         # the learned h state tiled over the rows
                 if self.cell_norm:
                     Bf['gst1_%d' % li] = self._z(S, NB, 4 * oc, 2)
                     Bf['gst2_%d' % li] = self._z(S, NB, oc, 2)
@@ -941,10 +1001,17 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if hp.nz:
             nz = hp.nz
             Bf['zs'] = self._z(S, NB, nz)             # zs fed to the two unrolls (posterior | prior)
-            Bf['zcat'] = self._z(S, NB, 2 * nz)       # [z_t, h_{t-1}] of the dense LSTM on z
-            Bf['zgates'] = self._z(S, NB, 4 * nz)
-            Bf['zc'] = self._z(S + 1, NB, nz)
-            Bf['zh'] = self._z(S + 1, NB, nz)
+            if self.z_cell in ('lstm', 'gru'):
+                Bf['zcat'] = self._z(S, NB, 2 * nz)   # [z_t, h_{t-1}] of the dense LSTM / the GRU's gates layer on z
+                Bf['zgates'] = self._z(S, NB, (4 if self.z_cell == 'lstm' else 2) * nz)
+                Bf['zh'] = self._z(S + 1, NB, nz)
+            if self.z_cell == 'lstm':
+                Bf['zc'] = self._z(S + 1, NB, nz)
+            elif self.z_cell == 'gru':
+                Bf['zccat'] = self._z(S, NB, 2 * nz)  # [z_t, r * h_{t-1}] of the candidate layer
+                Bf['zcand'] = self._z(S, NB, nz)
+            elif self.z_cell == 'fc':
+                Bf['zfc'] = self._z(S, NB, nz)        # dense(z) before the tanh
             self._build_posterior()
         self._plan_packs()
 
@@ -1183,21 +1250,58 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             L.copy_channels(src.data_ptr(), nz, zs[t, B:].data_ptr(), nz, B, nz)
 
     def _rnn_z_forward(self):
-        """Dense LSTM on z (savp_model.py:424-432): independent of the images, so the whole chain runs first
+        """The z cell (savp_model.py:424-432): independent of the images, so the whole chain runs first
         and every tile_concat of (actions, rnn_z) becomes one broadcast store per concat buffer."""
         hp = self.hparams
         Bf = self.Bf
         S, NB, nz, off = self.S, self.NB, hp.nz, self.A + self.Sd
         P = self.params
-        b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
         Zp = _ceil4(self.Zc)
-        Bf['zc'][0].zero_()
-        Bf['zh'][0].zero_()
+        zv = Bf['zvec'].data_ptr() + 4 * off
+        if self.z_cell is None:        # use_rnn_z=False: the zs are the rnn_z lanes
+            L.copy_channels(Bf['zs'].data_ptr(), nz, zv, Zp, S * NB, nz)
+            return
+        if self.z_cell == 'fc':        # fc_z: tanh(dense(z)) of every step at once
+            b = 'generator/rnn/savp_cell/fc_z/dense'
+            L.dense_fwd(Bf['zs'], nz, P[b + '/kernel'], P[b + '/bias'], Bf['zfc'], nz, S * NB, nz, nz)
+            L.act_fwd(Bf['zfc'].data_ptr(), nz, zv, Zp, S * NB, nz, L.ACT_TANH)
+            return
+        if self.z_cell == 'gru':
+            self._gru_z_forward()
+            return
+        b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
+        if hp.learn_initial_state:
+            self._load_initial_states(conv=False)
+        else:
+            Bf['zc'][0].zero_()
+            Bf['zh'][0].zero_()
         for t in range(S):
             L.copy_channels(Bf['zs'][t].data_ptr(), nz, Bf['zcat'][t].data_ptr(), 2 * nz, NB, nz)
             L.copy_channels(Bf['zh'][t].data_ptr(), nz, Bf['zcat'][t].data_ptr() + 4 * nz, 2 * nz, NB, nz)
             L.dense_fwd(Bf['zcat'][t], 2 * nz, P[b + '/kernel'], P[b + '/bias'], Bf['zgates'][t], 4 * nz, NB, 2 * nz, 4 * nz)
             L.lstm_cell_fwd(Bf['zgates'][t], Bf['zc'][t], Bf['zc'][t + 1], Bf['zh'][t + 1], NB, nz)
+            L.copy_channels(Bf['zh'][t + 1].data_ptr(), nz, Bf['zvec'][t].data_ptr() + 4 * off, Zp, NB, nz)
+
+    def _gru_z_forward(self):
+        """GRUCell on z (TF >= 1.9): r, u = sigmoid([z, h] Wg + bg); h' = u h + (1 - u) tanh([z, r h] Wc + bc)."""
+        Bf, P = self.Bf, self.params
+        S, NB, nz, off = self.S, self.NB, self.hparams.nz, self.A + self.Sd
+        b = 'generator/rnn/savp_cell/gru_z/gru_cell'
+        Zp = _ceil4(self.Zc)
+        if self.hparams.learn_initial_state:
+            self._load_initial_states(conv=False)
+        else:
+            Bf['zh'][0].zero_()
+        for t in range(S):
+            L.copy_channels(Bf['zs'][t].data_ptr(), nz, Bf['zcat'][t].data_ptr(), 2 * nz, NB, nz)
+            L.copy_channels(Bf['zh'][t].data_ptr(), nz, Bf['zcat'][t].data_ptr() + 4 * nz, 2 * nz, NB, nz)
+            L.dense_fwd(Bf['zcat'][t], 2 * nz, P[b + '/gates/kernel'], P[b + '/gates/bias'], Bf['zgates'][t], 2 * nz, NB, 2 * nz,
+                        2 * nz)
+            L.copy_channels(Bf['zs'][t].data_ptr(), nz, Bf['zccat'][t].data_ptr(), 2 * nz, NB, nz)
+            L.gru_cell_fwd(0, Bf['zgates'][t], Bf['zh'][t], None, Bf['zccat'][t].data_ptr() + 4 * nz, 2 * nz, None, NB, nz)
+            L.dense_fwd(Bf['zccat'][t], 2 * nz, P[b + '/candidate/kernel'], P[b + '/candidate/bias'], Bf['zcand'][t], nz, NB,
+                        2 * nz, nz)
+            L.gru_cell_fwd(1, Bf['zgates'][t], Bf['zh'][t], Bf['zcand'][t], 0, 0, Bf['zh'][t + 1], NB, nz)
             L.copy_channels(Bf['zh'][t + 1].data_ptr(), nz, Bf['zvec'][t].data_ptr() + 4 * off, Zp, NB, nz)
 
     def _state_pred_forward(self):
@@ -1232,7 +1336,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         d = self.gl[li]
         n_enc = len(self.enc_specs)
         dests = []
-        if d['use'] and t + 1 <= self.S:
+        if d['use'] and t + 1 <= self.S and not self.hparams.ablation_rnn:
             sp = d['rin_spec']
             dests.append((Bf['rin%d' % li][t + 1].data_ptr() + 4 * sp.off('h'), sp.cstride))
         if li + 1 < self.nl:
@@ -1270,8 +1374,16 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 self._site_conv(d['conv'], Bf['in%d' % li][t], pre, rin, rsp.off('x'), act=self.site_act)
                 self._site_norm(site, pre, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc, self.site_act, 0.0,
                                 Bf['nst%d' % li][t])
-                gpre = Bf['gpre%d' % li][t]
                 b = d['rname']
+                if hp.ablation_rnn:
+                    out = Bf['out%d' % li][t]
+                    self._site_conv(d['rconv'], rin, Bf['rpre%d' % li][t], out, act=self.site_act)
+                    self._site_norm(b, Bf['rpre%d' % li][t], out.data_ptr(), oc, NB, hh * ww, oc, self.site_act, 0.0,
+                                    Bf['rnst%d' % li][t])
+                    for addr, cs in self._h_dests(li, t):
+                        L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
+                    continue
+                gpre = Bf['gpre%d' % li][t]
                 if self.cell_norm:
                     d['rconv'].fwd(rin, gpre)
                     L.lstm_gates_fwd(gpre, NB, hh * ww, oc, Bf['c%d' % li][t],
@@ -1373,6 +1485,27 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         src = {'prev': self.Bf['img'][t], 'first': x[0], 'last': x[ctx - 1], 'last_context': x[t if t < ctx else ctx - 1]}
         return [(x[b[1]] if isinstance(b, tuple) else src[b]).data_ptr() for b in self.comp['bgs']]
 
+    def _load_initial_states(self, conv):
+        """The learned initial states (learn_initial_state), tiled over the NB rows into the t = 0 state buffers: the ConvLSTMs'
+        c[0] and the h slot of rin[0] (conv=True), or the z cell's zc[0] / zh[0] (conv=False).  Runs inside the step, so that a
+        captured graph reads the variables Adam has updated."""
+        Bf, NB = self.Bf, self.NB
+        for name, _, what, li in self._initial_state_specs():
+            if what.startswith('z') == conv:
+                continue
+            v = self.params[name]
+            n = v.numel()
+            if what in ('zc', 'zh', 'c'):
+                dst = Bf[what if what != 'c' else 'c%d' % li][0]
+                L.copy_channels(v.data_ptr(), 0, dst.data_ptr(), n, NB, n)
+                continue
+            d = self.gl[li]
+            sp = d['rin_spec']
+            h0 = Bf['h0_%d' % li]        # tiled [NB, hh, ww, oc], then into the strided h slot
+            L.copy_channels(v.data_ptr(), 0, h0.data_ptr(), n, NB, n)
+            L.copy_channels(h0.data_ptr(), d['oc'], Bf['rin%d' % li][0].data_ptr() + 4 * sp.off('h'), sp.cstride,
+                            NB * d['h'] * d['w'], d['oc'])
+
     def generator_forward(self, collect=True):
         hp = self.hparams
         if hp.nz:
@@ -1381,14 +1514,17 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         if self.Sd:
             self._state_pred_forward()
         self._broadcast_z()
-        for d in self.gl:
-            if d['use']:
-                li = d['li']
-                self.Bf['c%d' % li][0].zero_()
-                sp = d['rin_spec']
-                # h state entering step 0 is zero (zero_state, savp_model.py:344-352)
-                z = self.Bf['rin%d' % li][0]
-                z[..., sp.off('h'):sp.off('h') + d['oc']] = 0
+        if hp.learn_initial_state:
+            self._load_initial_states(conv=True)
+        else:
+            for d in self.gl:
+                if d['use'] and not hp.ablation_rnn:
+                    li = d['li']
+                    self.Bf['c%d' % li][0].zero_()
+                    sp = d['rin_spec']
+                    # h state entering step 0 is zero (zero_state, savp_model.py:344-352)
+                    z = self.Bf['rin%d' % li][0]
+                    z[..., sp.off('h'):sp.off('h') + d['oc']] = 0
         for t in range(self.S):
             self._gen_step(t)
         if collect:

@@ -231,10 +231,15 @@ class TrainMixin(object):
             li = d['li']
             G['din%d' % li] = torch.zeros_like(Bf['in%d' % li])
             G['dpre%d' % li] = torch.zeros_like(Bf['pre%d' % li])
-            if d['use']:
+            if d['use'] and hp.ablation_rnn:
+                G['drin%d' % li] = torch.zeros_like(Bf['rin%d' % li])
+                G['drpre%d' % li] = torch.zeros_like(Bf['rpre%d' % li])
+            elif d['use']:
                 G['drin%d' % li] = torch.zeros_like(Bf['rin%d' % li])
                 G['dgpre%d' % li] = torch.zeros_like(Bf['gpre%d' % li])
                 G['dc%d' % li] = torch.zeros_like(Bf['c%d' % li])
+                if 'h0_%d' % li in Bf:
+                    G['dh0_%d' % li] = torch.zeros_like(Bf['h0_%d' % li])
                 if 'hst%d' % li in Bf:       # ablation_conv_rnn_norm: gradient of the raw h from the downstream consumers
                     G['dhn%d' % li] = torch.zeros_like(Bf['out%d' % li])
         ngf = hp.ngf
@@ -260,10 +265,18 @@ class TrainMixin(object):
             G['dzvec'] = torch.zeros_like(Bf['zvec'])
         if hp.nz:
             nz = hp.nz
-            G['dzh'] = z(S + 1, NB, nz)        # gradient w.r.t. rnn_z h[t+1] (slot t+1)
-            G['dzc'] = z(S + 1, NB, nz)
-            G['dzgates'] = z(S, NB, 4 * nz)
-            G['dzcat'] = z(S, NB, 2 * nz)
+            if self.z_cell in ('lstm', 'gru'):
+                G['dzh'] = z(S + 1, NB, nz)        # gradient w.r.t. rnn_z h[t+1] (slot t+1)
+                G['dzgates'] = torch.zeros_like(Bf['zgates'])
+                G['dzcat'] = z(S, NB, 2 * nz)
+            if self.z_cell == 'lstm':
+                G['dzc'] = z(S + 1, NB, nz)
+            elif self.z_cell == 'gru':
+                G['dzcand'] = z(S, NB, nz)
+                G['dzccat'] = z(S, NB, 2 * nz)
+            elif self.z_cell == 'fc':
+                G['dzfc'] = z(S, NB, nz)
+                G['dzs'] = z(S, NB, nz)
             G['dzpost'] = z(S, self.B, nz)
             G['dzmu'] = z(S, self.B, nz)
             G['dzlss'] = z(S, self.B, nz)
@@ -420,7 +433,14 @@ class TrainMixin(object):
                 srcs.append((G['din%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
             if li == n_enc - 1 and self.cdna:
                 srcs.append((G['dsmall'][t].data_ptr(), oc))
-            if d['use'] and not self.cell_norm:
+            if d['use'] and hp.ablation_rnn:
+                # the conv_h site: its output's gradient through norm + activation and the 5x5 conv to (h{li} | z)
+                rsp = d['rin_spec']
+                self._site_norm_bwd(d['rname'], Bf['rpre%d' % li][t], Bf['out%d' % li][t].data_ptr(), oc, srcs, G['drpre%d' % li][t],
+                                    NB, hh * ww, oc, self.site_act, 0.0, Bf['rnst%d' % li][t])
+                d['rconv'].dgrad(G['drpre%d' % li][t], G['drin%d' % li][t])
+                srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
+            elif d['use'] and not self.cell_norm:
                 rsp = d['rin_spec']
                 if 'hst%d' % li in Bf:    # h -> IN(h) -> consumers: their gradient through the norm, before the recurrent one
                     nm_h = '%s/lstm_h%d/InstanceNorm' % (sc, li)
@@ -479,17 +499,19 @@ class TrainMixin(object):
         S, NB, B, H, W, C = self.S, self.NB, self.B, self.H, self.W, self.C
         rows_top = S * NB * H * W
         sc_cell = 'generator/rnn/savp_cell'
+        if hp.learn_initial_state:
+            self._initial_state_grads(conv=True)
         for d in self.gl:
             li = d['li']
             d['conv'].wgrad(Bf['in%d' % li], G['dpre%d' % li])
             L.colsum(G['dpre%d' % li].data_ptr(), d['oc'], Gp[d['conv'].bname], 1, S * NB * d['h'] * d['w'], d['oc'])
             if d['use']:
-                d['rconv'].wgrad(Bf['rin%d' % li][:S], G['dgpre%d' % li])
-                if d['rconv'].bname:      # norm-free cell: the gate convolution's bias
-                    L.colsum(G['dgpre%d' % li].data_ptr(), 4 * d['oc'], Gp[d['rconv'].bname], 1, S * NB * d['h'] * d['w'],
-                             4 * d['oc'])
+                dy = G['drpre%d' % li] if hp.ablation_rnn else G['dgpre%d' % li]
+                d['rconv'].wgrad(Bf['rin%d' % li][:S], dy)
+                if d['rconv'].bname:      # norm-free cell / conv_h site: the convolution's bias
+                    L.colsum(dy.data_ptr(), dy.shape[-1], Gp[d['rconv'].bname], 1, S * NB * d['h'] * d['w'], dy.shape[-1])
             if red is not None:
-                pre = ('%s/h%d/' % (sc_cell, li), '%s/lstm_h%d/' % (sc_cell, li))
+                pre = ('%s/h%d/' % (sc_cell, li), '%s/lstm_h%d/' % (sc_cell, li), '%s/conv_h%d/' % (sc_cell, li))
                 lo, hi = self._flat_range(self.g_flat, [k for k in P if k.startswith(pre)])
                 red.reduce_range(self.g_grad, lo, hi)
                 done.append((lo, hi))
@@ -535,21 +557,38 @@ class TrainMixin(object):
             return
         # the action and state slots' gradients are discarded: the states enter under stop_gradient (savp_model.py:414-421)
         nz, off = hp.nz, self.A + self.Sd
-        b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
-        G['dzh'].zero_()
-        for t in range(S - 1, -1, -1):
-            # dh[t+1] = z-slot gradient (rnn_z part) + recurrent part already accumulated in dzh[t+1]
-            L.axpy_channels(G['dzvec'][t].data_ptr() + 4 * off, Zp, G['dzh'][t + 1].data_ptr(), nz, NB, nz)
-            L.lstm_cell_bwd(Bf['zgates'][t], Bf['zc'][t], Bf['zc'][t + 1], G['dzh'][t + 1], G['dzc'][t + 1] if t + 1 < S else None,
-                            G['dzgates'][t], G['dzc'][t], NB, nz)
-            L.dense_bwd(Bf['zcat'][t], 2 * nz, P[b + '/kernel'], G['dzgates'][t], 4 * nz, NB, 2 * nz, 4 * nz, dx=G['dzcat'][t],
-                        dx_stride=2 * nz, dw=Gp[b + '/kernel'], dbias=Gp[b + '/bias'])
-            L.axpy_channels(G['dzcat'][t].data_ptr() + 4 * nz, 2 * nz, G['dzh'][t].data_ptr(), nz, NB, nz)
+        dzv = G['dzvec'].data_ptr() + 4 * off          # the rnn_z lanes of dzvec
+        if self.z_cell is None:      # use_rnn_z=False: dzs is the rnn_z lanes' gradient
+            dzs, dzs_cs = dzv, Zp
+        elif self.z_cell == 'fc':    # tanh(dense(z)): the tanh output is the rnn_z lanes of zvec
+            b = 'generator/rnn/savp_cell/fc_z/dense'
+            L.act_bwd(Bf['zvec'].data_ptr() + 4 * off, Zp, dzv, Zp, 0, 0, G['dzfc'].data_ptr(), nz, S * NB, nz, L.ACT_TANH)
+            L.dense_bwd(Bf['zs'], nz, P[b + '/kernel'], G['dzfc'], nz, S * NB, nz, nz, dx=G['dzs'], dx_stride=nz,
+                        dw=Gp[b + '/kernel'], dbias=Gp[b + '/bias'])
+            dzs, dzs_cs = G['dzs'].data_ptr(), nz
+        elif self.z_cell == 'gru':
+            self._gru_z_backward()
+            dzs, dzs_cs = G['dzcat'].data_ptr(), 2 * nz
+        else:
+            b = 'generator/rnn/savp_cell/lstm_z/basic_lstm_cell'
+            G['dzh'].zero_()
+            for t in range(S - 1, -1, -1):
+                # dh[t+1] = z-slot gradient (rnn_z part) + recurrent part already accumulated in dzh[t+1]
+                L.axpy_channels(G['dzvec'][t].data_ptr() + 4 * off, Zp, G['dzh'][t + 1].data_ptr(), nz, NB, nz)
+                L.lstm_cell_bwd(Bf['zgates'][t], Bf['zc'][t], Bf['zc'][t + 1], G['dzh'][t + 1], G['dzc'][t + 1] if t + 1 < S else None,
+                                G['dzgates'][t], G['dzc'][t], NB, nz)
+                L.dense_bwd(Bf['zcat'][t], 2 * nz, P[b + '/kernel'], G['dzgates'][t], 4 * nz, NB, 2 * nz, 4 * nz, dx=G['dzcat'][t],
+                            dx_stride=2 * nz, dw=Gp[b + '/kernel'], dbias=Gp[b + '/bias'])
+                L.axpy_channels(G['dzcat'][t].data_ptr() + 4 * nz, 2 * nz, G['dzh'][t].data_ptr(), nz, NB, nz)
+            dzs, dzs_cs = G['dzcat'].data_ptr(), 2 * nz
+        if hp.learn_initial_state:
+            self._initial_state_grads(conv=False)
         # dzs -> posterior sample: posterior half always, prior half for the context steps (savp_model.py:724-725)
         for t in range(S):
-            L.axpy_channels(G['dzcat'][t, :B].data_ptr(), 2 * nz, G['dzpost'][t].data_ptr(), nz, B, nz, accumulate=False)
+            row = dzs + 4 * t * NB * dzs_cs
+            L.axpy_channels(row, dzs_cs, G['dzpost'][t].data_ptr(), nz, B, nz, accumulate=False)
             if t < hp.context_frames - 1:
-                L.axpy_channels(G['dzcat'][t, B:].data_ptr(), 2 * nz, G['dzpost'][t].data_ptr(), nz, B, nz)
+                L.axpy_channels(row + 4 * B * dzs_cs, dzs_cs, G['dzpost'][t].data_ptr(), nz, B, nz)
         L.sample_z_bwd(Bf['zmu'], Bf['zlss'], Bf['eps'], G['dzpost'], G['dzmu'], G['dzlss'], S * B * nz, self.step_scalars[2:3])
         sc = 'generator/encoder'
         last = self.enc_layers[-1]
@@ -580,6 +619,44 @@ class TrainMixin(object):
                 x_in = Bf['pairs']
             el['conv'].wgrad(x_in, G['depre%d' % i])
             L.colsum(G['depre%d' % i].data_ptr(), oc, Gp[el['conv'].bname], 1, S * B * pos, oc)
+
+    def _initial_state_grads(self, conv):
+        """Gradients of the learned initial states: the sum over the NB rows of the t = 0 state gradient -- dc[0] and the h
+        slot of drin[0] of the ConvLSTMs (conv=True), dzc[0] / dzh[0] of the z cell (conv=False)."""
+        G, Gp, NB = self.Gb, self.grads, self.NB
+        for name, _, what, li in self._initial_state_specs():
+            if what.startswith('z') == conv:
+                continue
+            n = self.params[name].numel()
+            if what in ('zc', 'zh', 'c'):
+                src = G['d' + what if what != 'c' else 'dc%d' % li][0]
+            else:
+                d = self.gl[li]
+                sp = d['rin_spec']
+                src = G['dh0_%d' % li]       # the strided h slot made contiguous per row
+                L.copy_channels(G['drin%d' % li][0].data_ptr() + 4 * sp.off('h'), sp.cstride, src.data_ptr(), d['oc'],
+                                NB * d['h'] * d['w'], d['oc'])
+            L.colsum(src.data_ptr(), n, Gp[name], 1, NB, n)
+
+    def _gru_z_backward(self):
+        """BPTT through the GRU on z (savp_model._gru_z_forward); leaves dL/dzs in the z lanes of dzcat."""
+        Bf, G, P, Gp = self.Bf, self.Gb, self.params, self.grads
+        S, NB, nz = self.S, self.NB, self.hparams.nz
+        Zp, off = _ceil4(self.Zc), self.A + self.Sd
+        b = 'generator/rnn/savp_cell/gru_z/gru_cell'
+        G['dzh'].zero_()
+        for t in range(S - 1, -1, -1):
+            L.axpy_channels(G['dzvec'][t].data_ptr() + 4 * off, Zp, G['dzh'][t + 1].data_ptr(), nz, NB, nz)
+            L.gru_cell_bwd(0, Bf['zgates'][t], Bf['zh'][t], Bf['zcand'][t], G['dzh'][t + 1], 0, 0, G['dzgates'][t], G['dzcand'][t],
+                           G['dzh'][t], NB, nz)
+            L.dense_bwd(Bf['zccat'][t], 2 * nz, P[b + '/candidate/kernel'], G['dzcand'][t], nz, NB, 2 * nz, nz, dx=G['dzccat'][t],
+                        dx_stride=2 * nz, dw=Gp[b + '/candidate/kernel'], dbias=Gp[b + '/candidate/bias'])
+            L.gru_cell_bwd(1, Bf['zgates'][t], Bf['zh'][t], None, None, G['dzccat'][t].data_ptr() + 4 * nz, 2 * nz, G['dzgates'][t],
+                           None, G['dzh'][t], NB, nz)
+            L.dense_bwd(Bf['zcat'][t], 2 * nz, P[b + '/gates/kernel'], G['dzgates'][t], 2 * nz, NB, 2 * nz, 2 * nz, dx=G['dzcat'][t],
+                        dx_stride=2 * nz, dw=Gp[b + '/gates/kernel'], dbias=Gp[b + '/gates/bias'])
+            L.axpy_channels(G['dzcat'][t].data_ptr() + 4 * nz, 2 * nz, G['dzh'][t].data_ptr(), nz, NB, nz)
+            L.axpy_channels(G['dzccat'][t].data_ptr(), 2 * nz, G['dzcat'][t].data_ptr(), 2 * nz, NB, nz)
 
     # ------------------------------------------------------------------ one optimisation step
     def loss_slots(self):

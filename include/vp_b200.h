@@ -111,6 +111,19 @@ int vp_tf32_residual(const float* x, float* lo, long long n, vp_stream_t stream)
 int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked, int n_pad,
                   int kc, int split_k, vp_stream_t stream);
 
+/* The form vp_conv_wgrad launches for a call of this shape on a device with `sms` SMs: its index among
+ * vp_conv_wgrad_forms, the CTA count, the pixel-range split count and the 64-pixel stages per CTA.  x_ndhwc / dy_ndhwc =
+ * the operands' {n, d, h, w, c}; g, n_pad, kc and split_k as passed to the call.  The split count depends on the layer
+ * alone, the form on the shape alone. */
+int vp_conv_wgrad_form(const vp_conv_geom* g, const int x_ndhwc[5], const int dy_ndhwc[5], int n_pad, int kc, int split_k,
+                       int sms, int* form, int* ctas, int* splits, int* stages_per_cta);
+/* The forms of vp_conv_wgrad, into blocks[i] (32-row blocks of taps x channel chunks per CTA), bn[i] (GEMM columns) for
+ * i < min(count, cap); returns the count. */
+int vp_conv_wgrad_forms(int* blocks, int* bn, int cap);
+/* vp_conv_wgrad in the given form (for comparing forms): the same sums in the same order, so the same bits. */
+int vp_conv_wgrad_in_form(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked, int n_pad,
+                          int kc, int split_k, int form, vp_stream_t stream);
+
 /* Weight packing: reference-layout kernel w [kd][kh][kw][ci_ref][co] (HWIO / DHWIO) ->
  * effective tap matrices in tensor-core layout, TF32-rounded.
  *  kind PLAIN:     taps = kd*kh*kw, Keff = w

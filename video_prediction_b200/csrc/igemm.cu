@@ -295,15 +295,15 @@ __global__ void __launch_bounds__(kFwdThreads, 1) igemm_fwd_kernel(const __grid_
 // wgrad_xt_kernel copies the plain operand once per call into scratch as T[c][pixel], channel-major, pixels in the main
 // kernel's 64-pixel tile order and zero outside the lattice: a K-major wgmma B operand (N = plain channels, K = pixels),
 // fetched with 32-pixel x BN-channel TMA boxes (channels past the view are TMA zero fill).  The filter taps are folded into
-// GEMM-M: a CTA owns four 32-row blocks, each a (tap, 32-channel chunk of the shifted operand) pair whose rows are a 5-D
+// GEMM-M: a CTA owns kBlocks 32-row blocks, each a (tap, 32-channel chunk of the shifted operand) pair whose rows are a 5-D
 // TMA box of the tap's parity lattice at the tap's shift (channel-minor, 128B swizzle, zero fill = the padding), so one B
-// tile per 64 pixels serves all of a CTA's taps.  Each thread loads its A fragments from the box with lds and issues
-// wgmma.m64nBNk8 in the register-A form.  The products of a dW element are summed in pixel order, 8 pixels per MMA, over
-// the tiles of its pixel-range split.
+// tile per 64 pixels serves all of a CTA's taps.  With four blocks each consumer warpgroup owns two of them and all BN
+// columns; with two both warpgroups read the same two blocks and each owns BN / 2 of the columns.  Each thread loads its A
+// fragments from the box with lds and issues wgmma.m64nNk8 in the register-A form.  The products of a dW element are
+// summed in pixel order, 8 pixels per MMA, over the tiles of its pixel-range split, whatever the form.
 // ------------------------------------------------------------------------------------------------
 constexpr int kWgTile = 64;        // pixels (GEMM-K) per pipeline stage
-constexpr int kWgBlocks = 4;       // 32-row (tap, channel chunk) blocks per CTA: two per consumer warpgroup
-constexpr int kWgMaxStages = 6;
+constexpr int kWgMaxStages = 8;
 constexpr int kWgThreads = 384;
 
 struct alignas(64) WgradArgs {
@@ -325,19 +325,38 @@ struct alignas(64) WgradArgs {
 // banks for the four pixel rows t = 0..3 (a contiguous 8 channels would be a 2-way conflict).
 __device__ __forceinline__ int wg_row_channel(int rho) { return 4 * (rho >> 3) + (rho & 3) + 16 * ((rho >> 2) & 1); }
 
-template <int BN>
+// The A fragments of one stage: k = 8 ks + t (+ 4) is the pixel row, and under the 128B swizzle (k & 7) does not depend on
+// ks, so each of the 32 loads is one of four per-thread offsets `fo` plus ks KB.
+__device__ __forceinline__ void wg_load_frags(uint32_t (&af)[8][4], uint32_t ab, const uint32_t (&fo)[4], bool live) {
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) af[ks][q] = live ? lds_u32(ab + 1024u * ks + fo[q]) : 0u;
+}
+
+template <int N, uint32_t kTHalf>
+__device__ __forceinline__ void wg_issue(float (&acc)[N / 2], const uint32_t (&af)[8][4], uint64_t bd) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) WgmmaRS<N>::mma(acc, af[ks], bd + (ks < 4 ? 2 * ks : kTHalf / 16 + 2 * (ks - 4)));
+  wgmma_commit();
+}
+
+template <int BN, int kBlocks>
 __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid_constant__ WgradArgs a) {
+  static_assert(kBlocks == 4 || (kBlocks == 2 && BN % 16 == 0), "two-block tiles split BN into two wgmma N");
+  constexpr int kWN = kBlocks == 4 ? BN : BN / 2;           // wgmma N of one consumer warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ uint64_t full_bar[kWgMaxStages], empty_bar[kWgMaxStages];
   constexpr uint32_t kBox = kWgTile * 128;                  // one row block: 64 pixels x 32 channels
   constexpr uint32_t kTHalf = BN * 128;                     // 32 pixels of the B tile: BN channel rows of 128 B
-  constexpr uint32_t kStage = kWgBlocks * kBox + 2 * kTHalf;
+  constexpr uint32_t kStage = kBlocks * kBox + 2 * kTHalf;
 
   const int wg = threadIdx.x >> 7;
   const int ntile = blockIdx.x % a.n_tiles;
-  const int blk0 = (blockIdx.x / a.n_tiles) * kWgBlocks;
-  const int nblk = min(kWgBlocks, a.num_taps * a.chunks - blk0);
+  const int blk0 = (blockIdx.x / a.n_tiles) * kBlocks;
+  const int nblk = min(kBlocks, a.num_taps * a.chunks - blk0);
   const int c0 = ntile * BN;
   const int total = a.tiles_w * a.tiles_h * a.tiles_d * a.tiles_n;
   const int it0 = static_cast<int>(static_cast<long long>(total) * blockIdx.y / a.splits);
@@ -354,6 +373,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid
   const uint32_t full0 = smem_u32(&full_bar[0]), empty0 = smem_u32(&empty_bar[0]);
   const uint32_t ring_end = static_cast<uint32_t>(a.stages) * 8u;
   if (wg == 0) {
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int rem = it0;
       int tw = rem % a.tiles_w; rem /= a.tiles_w;
@@ -373,8 +393,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid
           const Tap tp = a.taps[b / a.chunks];
           tma_load_5d_addr(dst + j * kBox, &a.amap[tp.map], fb, 32 * (b % a.chunks), x0 + tp.cw, y0 + tp.ch, d0 + tp.cd, s0);
         }
-        tma_load_2d_addr(dst + kWgBlocks * kBox, &a.tmap, fb, it * kWgTile, c0);
-        tma_load_2d_addr(dst + kWgBlocks * kBox + kTHalf, &a.tmap, fb, it * kWgTile + 32, c0);
+        tma_load_2d_addr(dst + kBlocks * kBox, &a.tmap, fb, it * kWgTile, c0);
+        tma_load_2d_addr(dst + kBlocks * kBox + kTHalf, &a.tmap, fb, it * kWgTile + 32, c0);
         if (++tw == a.tiles_w) { tw = 0; if (++th == a.tiles_h) { th = 0; if (++td == a.tiles_d) { td = 0; ++tn; } } }
         s_off += kStage; b_off += 8;
         if (b_off == ring_end) { s_off = 0; b_off = 0; ph ^= 1; }
@@ -383,43 +403,60 @@ __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid
     return;
   }
 
-  // ---- consumers: warpgroup h owns row blocks 2h, 2h + 1; warp w of it rows 16 (w % 2) .. + 15 of block 2h + w / 2
+  // ---- consumers.  Four blocks: warpgroup h owns row blocks 2h, 2h + 1 and all BN columns; two blocks: both warpgroups
+  // own blocks 0, 1 and warpgroup h columns h BN / 2 .. + BN / 2 - 1 (a whole number of 1024-byte swizzle atoms into the
+  // B tile).  Warp w of a warpgroup holds rows 16 (w % 2) .. + 15 of its block j.
+  setmaxnreg_inc<232>();
   const int h = wg - 1, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int j = 2 * h + (w >> 1);
+  const int j = kBlocks == 4 ? 2 * h + (w >> 1) : (w >> 1);
+  const int col0 = kBlocks == 4 ? 0 : h * kWN;
   const bool live = j < nblk;
   const int c_lo = wg_row_channel(16 * (w & 1) + g), c_hi = wg_row_channel(16 * (w & 1) + 8 + g);
-  const uint64_t bd_base = make_wgmma_desc(smem0 + kWgBlocks * kBox, 16, 1024, kWgmmaSwizzle128B);
-  float acc[BN / 2];
+  const uint32_t fo[4] = {sw128_offset(t, c_lo), sw128_offset(t, c_hi), sw128_offset(t + 4, c_lo), sw128_offset(t + 4, c_hi)};
+  const uint32_t a_base = smem0 + static_cast<uint32_t>(j) * kBox;
+  const uint64_t bd_base = make_wgmma_desc(smem0 + kBlocks * kBox + col0 * 128u, 16, 1024, kWgmmaSwizzle128B);
+  float acc[kWN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  uint32_t s_off = 0, b_off = 0, ph = 0;
+  for (int i = 0; i < kWN / 2; ++i) acc[i] = 0.f;
+  // Two fragment sets, the loop unrolled by two so that each stays in fixed registers.  After committing stage i the
+  // group of stage i - 1 is waited for (one group stays in flight), its stage released, and stage i + 1's fragments
+  // loaded into the set that group has finished reading: the lds of a stage overlap the MMAs of the previous one.
+  uint32_t fa[8][4], fb[8][4];
+  uint32_t s_off = 0, b_off = 0, ph = 0, held = 0;
+  mbar_wait_addr(full0, 0);
+  wg_load_frags(fa, a_base, fo, live);
+  int it = it0;
 #pragma unroll 1
-  for (int it = it0; it < it1; ++it) {
-    mbar_wait_addr(full0 + b_off, ph);
-    uint32_t af[8][4];
-    const uint32_t ab = smem0 + s_off + static_cast<uint32_t>(j) * kBox;
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      const int k = 8 * ks + t;
-      af[ks][0] = live ? lds_u32(ab + sw128_offset(k, c_lo)) : 0u;
-      af[ks][1] = live ? lds_u32(ab + sw128_offset(k, c_hi)) : 0u;
-      af[ks][2] = live ? lds_u32(ab + sw128_offset(k + 4, c_lo)) : 0u;
-      af[ks][3] = live ? lds_u32(ab + sw128_offset(k + 4, c_hi)) : 0u;
+  for (;;) {
+    wg_issue<kWN, kTHalf>(acc, fa, bd_base + (s_off >> 4));
+    wgmma_wait<1>();
+    if (it > it0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive_addr(empty0 + held);
     }
-    const uint64_t bd = bd_base + (s_off >> 4);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks)
-      WgmmaRS<BN>::mma(acc, af[ks], bd + (ks < 4 ? 2 * ks : kTHalf / 16 + 2 * (ks - 4)));
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_acc(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive_addr(empty0 + b_off);
+    held = b_off;
     s_off += kStage; b_off += 8;
     if (b_off == ring_end) { s_off = 0; b_off = 0; ph ^= 1; }
+    if (++it == it1) break;
+    mbar_wait_addr(full0 + b_off, ph);
+    wg_load_frags(fb, a_base + s_off, fo, live);
+
+    wg_issue<kWN, kTHalf>(acc, fb, bd_base + (s_off >> 4));
+    wgmma_wait<1>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive_addr(empty0 + held);
+    held = b_off;
+    s_off += kStage; b_off += 8;
+    if (b_off == ring_end) { s_off = 0; b_off = 0; ph ^= 1; }
+    if (++it == it1) break;
+    mbar_wait_addr(full0 + b_off, ph);
+    wg_load_frags(fa, a_base + s_off, fo, live);
   }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  __syncwarp();
+  if (lane == 0) mbar_arrive_addr(empty0 + held);
   if (!live) return;
   // every dW element has one owner per pixel-range split, which adds its sum without atomics: into dW itself when there is
   // one split, otherwise into the split's own zero-filled scratch plane, which reduce_parts adds to dW in split order
@@ -431,10 +468,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) igemm_wgrad_kernel(const __grid
     const int row = 32 * (b % a.chunks) + (r ? c_hi : c_lo);
     if (row >= a.rows_valid) continue;
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
+    for (int i = 0; i < kWN / 8; ++i) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int col = c0 + 8 * i + 2 * t + e;
+        const int col = c0 + col0 + 8 * i + 2 * t + e;
         if (col >= a.cols_valid) continue;
         // dW is [co][ci]: GEMM rows are x channels (ci) for a conv and dy channels (co) for a transposed conv
         float* o = a.rows_are_ci ? plane + static_cast<long long>(col) * a.kpad + row : plane + static_cast<long long>(row) * a.kpad + col;
@@ -823,13 +860,65 @@ extern "C" int vp_conv_lstm_fwd(const vp_tensor* in, const vp_conv_geom* g, cons
   return conv_igemm_impl(in, g, wpacked, n_pad, kc, z, bias, VP_ACT_NONE, 0.f, 1, accumulate, nullptr, nullptr, 0, stream, &cell);
 }
 
-extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked,
-                             int n_pad, int kc, int split_k, vp_stream_t stream) {
-  if (check_tensor(x, "vp_conv_wgrad(x)") || check_tensor(dy, "vp_conv_wgrad(dy)")) return -1;
-  if (!g || !dwpacked) return set_error("vp_conv_wgrad: null argument");
+typedef void (*WgKernel)(const WgradArgs);
+struct WgradForm {
+  int blocks, bn;      // 32-row blocks (taps x channel chunks of the shifted operand) x GEMM columns of a CTA
+  float stage_us;      // time of one 64-pixel stage of one CTA with every SM busy
+  WgKernel kernel;
+};
+// Forms of igemm_wgrad_kernel.  stage_us is the median over the 21 distinct weight-gradient calls of the cfg2 training
+// step of (call time) / (waves x stages per CTA), each call timed in every form (tests/measure_wgrad_forms.py: CUDA graphs
+// of 10 calls on fresh operands, median of 5 replays; NVIDIA H100 80GB HBM3, 700 W power limit, 1980 MHz max SM clock).
+// With these costs pick_wgrad_form chooses the fastest form of every one of those calls.  BN = 16 serves the output
+// convolutions with co <= 8; BN = 72 and 136 exist only with four blocks (BN / 2 is not a whole swizzle atom).
+static const WgradForm kWgradForms[] = {
+    {4, 16, 1.108f, igemm_wgrad_kernel<16, 4>},   {4, 32, 1.199f, igemm_wgrad_kernel<32, 4>},
+    {4, 64, 1.375f, igemm_wgrad_kernel<64, 4>},   {4, 72, 1.428f, igemm_wgrad_kernel<72, 4>},
+    {4, 128, 1.652f, igemm_wgrad_kernel<128, 4>}, {4, 136, 1.671f, igemm_wgrad_kernel<136, 4>},
+    {2, 16, 0.698f, igemm_wgrad_kernel<16, 2>},   {2, 32, 0.766f, igemm_wgrad_kernel<32, 2>},
+    {2, 64, 0.849f, igemm_wgrad_kernel<64, 2>},   {2, 128, 1.066f, igemm_wgrad_kernel<128, 2>},
+};
+constexpr int kNumWgradForms = static_cast<int>(sizeof(kWgradForms) / sizeof(kWgradForms[0]));
+
+static int wgrad_ctas(const WgradForm& f, int nblocks, int plain_c, int splits) {
+  return ceil_div(nblocks, f.blocks) * ceil_div(plain_c, f.bn) * splits;
+}
+
+// The form of a weight-gradient call, from its shape alone: the one with the least estimated time, waves of CTAs x
+// stages per CTA x the form's cost per stage (ties: the earlier form).  `nblocks` = taps x 32-channel chunks of the
+// shifted operand, `plain_c` = channels of the other operand (GEMM-N).
+static int pick_wgrad_form(int nblocks, int plain_c, int splits, int stages, int sms) {
+  int best = 0;
+  double best_t = 1e30;
+  for (int f = 0; f < kNumWgradForms; ++f) {
+    const double waves = ceil_div(wgrad_ctas(kWgradForms[f], nblocks, plain_c, splits), sms);
+    const double t = waves * stages * kWgradForms[f].stage_us;
+    if (t < best_t) { best_t = t; best = f; }
+  }
+  return best;
+}
+
+// Four blocks and the N tile (32, 64, 72, 128 or 136) that covers `plain_c` channels with the fewest padded columns (ties:
+// the wider): the form of the 3-D calls.  Those run inside the concurrent discriminator towers of the training step, whose
+// results differ from run to run when the towers' timing shifts (DESIGN.md, weight gradient), so they keep the timing of
+// this form until that is found.
+static int padding_form(int plain_c) {
+  int best = 1, best_cols = 1 << 30;
+  for (int f = kNumWgradForms - 1; f >= 0; --f) {
+    const WgradForm& fm = kWgradForms[f];
+    if (fm.blocks != 4 || fm.bn == 16) continue;
+    const int cols = ceil_div(plain_c, fm.bn) * fm.bn;
+    if (cols < best_cols) { best_cols = cols; best = f; }
+  }
+  return best;
+}
+
+// Taps, pixel tiles, pixel-range splits and stage count of a weight-gradient call into A; returns the index of its form in
+// kWgradForms (`form` if that is >= 0), -1 on error.  Only the extents and channel counts of the operands are read.
+static int plan_wgrad(WgradArgs& A, const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, int n_pad, int kc,
+                      int split_k, int sms, int form) {
   if (n_pad % 16 || dy->c > n_pad || kc * 32 < x->c) return set_error("vp_conv_wgrad: bad n_pad / kc");
-  static thread_local WgradArgs A;
-  std::memset(&A, 0, sizeof(A));
+  if (form >= kNumWgradForms) return set_error("vp_conv_wgrad: no form %d", form);
   // conv:  dW[r] += sum_o x[s*o+r-p]^T dy[o]   (x shifted, lattice = dy)
   // tconv: dW[r] += sum_o dy[s*o+r-p]^T x[o]   (dy shifted, lattice = x); as a gather this is a plain (non-transposed)
   //        strided access pattern, so the taps are those of the geometry with transposed = 0.
@@ -849,37 +938,50 @@ extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_c
   A.tiles_d = ceil_div(plain->d, A.bd); A.tiles_n = ceil_div(plain->n, A.bn);
   const long long total = static_cast<long long>(A.tiles_w) * A.tiles_h * A.tiles_d * A.tiles_n;
   if (total * kWgTile > (1LL << 31) - 1) return set_error("vp_conv_wgrad: too many pixels");
-  const int box[4] = {A.bw, A.bh, A.bd, A.bn};
-  for (int qd = 0; qd < g->sd; ++qd)
-    for (int qh = 0; qh < g->sh; ++qh)
-      for (int qw = 0; qw < g->sw; ++qw)
-        if (make_act_map(&A.amap[(qd * g->sh + qh) * g->sw + qw], shifted, qd, qh, qw, g->sd, g->sh, g->sw, box)) return -1;
   A.chunks = ceil_div(shifted->c, 32);
   A.rows_valid = shifted->c; A.cols_valid = plain->c;
   A.rows_are_ci = g->transposed ? 0 : 1;
   A.n_pad = n_pad; A.kpad = kc * 32;
-  const int m_tiles = ceil_div(ntaps * A.chunks, kWgBlocks);
-  // N tile (GEMM-N = plain channels): the wgmma N whose tiles cover them with the fewest padded columns (ties: the wider)
-  int bn_tile = 32;
-  {
-    int best = 1 << 30;
-    for (int bn : {136, 128, 72, 64, 32}) {
-      const int cols = ceil_div(plain->c, bn) * bn;
-      if (cols < best) { best = cols; bn_tile = bn; }
-    }
-  }
-  A.n_tiles = ceil_div(plain->c, bn_tile);
-  const size_t stage_bytes = static_cast<size_t>(kWgBlocks) * kWgTile * 128 + 2 * static_cast<size_t>(bn_tile) * 128;
-  const size_t smem_max = 227 * 1024 - 2048;
-  A.stages = static_cast<int>(std::min<size_t>(kWgMaxStages, (smem_max - 1024) / stage_bytes));
   // The pixel range is split by a rule of the layer's shape alone -- two waves of (taps x 128-row dy tiles x 128-column x
   // tiles) CTAs, at least four tiles per split -- not of the kernel's tiling, so the grouping of every dW sum (and with
   // it the fp32 result) depends only on the layer.
   if (split_k <= 0) {
     const int ctas = ntaps * ceil_div(std::min(n_pad, ceil_div(dy->c, 32) * 32), 128) * ceil_div(kc, 4);
-    split_k = std::max(1, (2 * device_sms()) / ctas);
+    split_k = std::max(1, (2 * sms) / ctas);
   }
   A.splits = static_cast<int>(std::max<long long>(1, std::min<long long>(split_k, std::max<long long>(1, total / 4))));
+  const int stages = static_cast<int>(ceil_div(static_cast<int>(total), A.splits));
+  const int f = form >= 0 ? form
+               : plain->d > 1 || shifted->d > 1 ? padding_form(plain->c)
+                                                : pick_wgrad_form(ntaps * A.chunks, plain->c, A.splits, stages, sms);
+  A.n_tiles = ceil_div(plain->c, kWgradForms[f].bn);
+  return f;
+}
+
+static size_t wgrad_stage_bytes(const WgradForm& f) {
+  return static_cast<size_t>(f.blocks) * kWgTile * 128 + 2 * static_cast<size_t>(f.bn) * 128;
+}
+
+static int conv_wgrad_impl(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked, int n_pad,
+                           int kc, int split_k, int form, vp_stream_t stream) {
+  if (check_tensor(x, "vp_conv_wgrad(x)") || check_tensor(dy, "vp_conv_wgrad(dy)")) return -1;
+  if (!g || !dwpacked) return set_error("vp_conv_wgrad: null argument");
+  static thread_local WgradArgs A;
+  std::memset(&A, 0, sizeof(A));
+  const int f = plan_wgrad(A, x, dy, g, n_pad, kc, split_k, device_sms(), form);
+  if (f < 0) return -1;
+  const WgradForm& fm = kWgradForms[f];
+  const vp_tensor* shifted = g->transposed ? dy : x;
+  const vp_tensor* plain = g->transposed ? x : dy;
+  const long long total = static_cast<long long>(A.tiles_w) * A.tiles_h * A.tiles_d * A.tiles_n;
+  const int box[4] = {A.bw, A.bh, A.bd, A.bn};
+  for (int qd = 0; qd < g->sd; ++qd)
+    for (int qh = 0; qh < g->sh; ++qh)
+      for (int qw = 0; qw < g->sw; ++qw)
+        if (make_act_map(&A.amap[(qd * g->sh + qh) * g->sw + qw], shifted, qd, qh, qw, g->sd, g->sh, g->sw, box)) return -1;
+  const size_t stage_bytes = wgrad_stage_bytes(fm);
+  const size_t smem_max = 227 * 1024 - 2048;
+  A.stages = static_cast<int>(std::min<size_t>(kWgMaxStages, (smem_max - 1024) / stage_bytes));
 
   TransposeArgs T;
   std::memset(&T, 0, sizeof(T));
@@ -896,7 +998,7 @@ extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_c
     if (!enc) { scratch_free(tbuf, stream); return set_error("cuTensorMapEncodeTiled entry point not found"); }
     cuuint64_t dims[2] = {static_cast<cuuint64_t>(T.p_pad), static_cast<cuuint64_t>(plain->c)};
     cuuint64_t strides[1] = {static_cast<cuuint64_t>(T.p_pad) * 4};
-    cuuint32_t boxd[2] = {32, static_cast<cuuint32_t>(bn_tile)};
+    cuuint32_t boxd[2] = {32, static_cast<cuuint32_t>(fm.bn)};
     cuuint32_t es[2] = {1, 1};
     CUresult r = enc(&A.tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, tbuf, dims, strides, boxd, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -905,26 +1007,23 @@ extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_c
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   wgrad_transpose_kernel<<<dim3(static_cast<unsigned>(total), ceil_div(plain->c, 32)), 256, 0, st>>>(T);
   int rc = check_launch("wgrad_transpose_kernel");
-  const long long plane = static_cast<long long>(ntaps) * n_pad * A.kpad;
+  const long long plane = static_cast<long long>(A.num_taps) * n_pad * A.kpad;
   float* ws = nullptr;
   if (!rc && A.splits > 1) rc = scratch_zeroed(&ws, A.splits * plane, stream);
   if (!rc) {
     A.out = A.splits > 1 ? ws : dwpacked;
     A.so_n = plane;
-    typedef void (*WgKernel)(const WgradArgs);
-    static const WgKernel kernels[5] = {igemm_wgrad_kernel<32>, igemm_wgrad_kernel<64>, igemm_wgrad_kernel<72>,
-                                        igemm_wgrad_kernel<128>, igemm_wgrad_kernel<136>};
     static bool attr_set = false;
     if (!attr_set) {
-      for (WgKernel k : kernels)
-        if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
+      for (const WgradForm& k : kWgradForms)
+        if (cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_max)) != cudaSuccess)
           rc = set_error("cudaFuncSetAttribute(igemm_wgrad_kernel) failed: %s", cudaGetErrorString(cudaGetLastError()));
       attr_set = rc == 0;
     }
     if (!rc) {
-      const WgKernel kernel = kernels[bn_tile == 32 ? 0 : bn_tile == 64 ? 1 : bn_tile == 72 ? 2 : bn_tile == 128 ? 3 : 4];
       const size_t smem = static_cast<size_t>(A.stages) * stage_bytes + 1024;
-      kernel<<<dim3(m_tiles * A.n_tiles, A.splits), kWgThreads, smem, st>>>(A);
+      const int m_tiles = ceil_div(A.num_taps * A.chunks, fm.blocks);
+      fm.kernel<<<dim3(m_tiles * A.n_tiles, A.splits), kWgThreads, smem, st>>>(A);
       rc = check_launch("igemm_wgrad_kernel");
     }
   }
@@ -934,4 +1033,38 @@ extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_c
   }
   scratch_free(tbuf, stream);
   return rc;
+}
+
+extern "C" int vp_conv_wgrad(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked,
+                             int n_pad, int kc, int split_k, vp_stream_t stream) {
+  return conv_wgrad_impl(x, dy, g, dwpacked, n_pad, kc, split_k, -1, stream);
+}
+
+extern "C" int vp_conv_wgrad_in_form(const vp_tensor* x, const vp_tensor* dy, const vp_conv_geom* g, float* dwpacked,
+                                     int n_pad, int kc, int split_k, int form, vp_stream_t stream) {
+  if (form < 0) return set_error("vp_conv_wgrad_in_form: no form %d", form);
+  return conv_wgrad_impl(x, dy, g, dwpacked, n_pad, kc, split_k, form, stream);
+}
+
+extern "C" int vp_conv_wgrad_form(const vp_conv_geom* g, const int x_ndhwc[5], const int dy_ndhwc[5], int n_pad, int kc,
+                                  int split_k, int sms, int* form, int* ctas, int* splits, int* stages_per_cta) {
+  if (!g || !x_ndhwc || !dy_ndhwc || !form || !ctas || !splits || !stages_per_cta || sms < 1 || kc < 1)
+    return set_error("vp_conv_wgrad_form: bad argument");
+  static thread_local WgradArgs A;
+  std::memset(&A, 0, sizeof(A));
+  const vp_tensor x{nullptr, x_ndhwc[0], x_ndhwc[1], x_ndhwc[2], x_ndhwc[3], x_ndhwc[4], x_ndhwc[4]};
+  const vp_tensor dy{nullptr, dy_ndhwc[0], dy_ndhwc[1], dy_ndhwc[2], dy_ndhwc[3], dy_ndhwc[4], dy_ndhwc[4]};
+  const int f = plan_wgrad(A, &x, &dy, g, n_pad, kc, split_k, sms, -1);
+  if (f < 0) return -1;
+  const long long total = static_cast<long long>(A.tiles_w) * A.tiles_h * A.tiles_d * A.tiles_n;
+  *form = f;
+  *ctas = wgrad_ctas(kWgradForms[f], A.num_taps * A.chunks, A.cols_valid, A.splits);
+  *splits = A.splits;
+  *stages_per_cta = static_cast<int>((total + A.splits - 1) / A.splits);
+  return 0;
+}
+
+extern "C" int vp_conv_wgrad_forms(int* blocks, int* bn, int cap) {
+  for (int f = 0; f < kNumWgradForms && f < cap; ++f) { blocks[f] = kWgradForms[f].blocks; bn[f] = kWgradForms[f].bn; }
+  return kNumWgradForms;
 }

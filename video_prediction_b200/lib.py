@@ -214,6 +214,29 @@ def conv_wgrad(x_view, dy_view, g, dwpacked, n_pad, kc, split_k=1):
                                                                split_k, stream_ptr())))
 
 
+def conv_wgrad_in_form(x_view, dy_view, g, dwpacked, n_pad, kc, split_k, form):
+    """conv_wgrad in form `form` (an index into conv_wgrad_forms()) instead of the one the call's shape selects."""
+    check(lib().vp_conv_wgrad_in_form(C.byref(x_view), C.byref(dy_view), C.byref(g), ptr(dwpacked), n_pad, kc, split_k,
+                                      form, stream_ptr()))
+
+
+def conv_wgrad_form(g, x_ndhwc, dy_ndhwc, n_pad, kc, sms, split_k=1):
+    """(form index, CTAs, pixel-range splits, 64-pixel stages per CTA) of the conv_wgrad call of this shape on `sms` SMs;
+    x_ndhwc / dy_ndhwc = the operands' (n, d, h, w, c).  Needs no device."""
+    out = [C.c_int() for _ in range(4)]
+    check(lib().vp_conv_wgrad_form(C.byref(g), (C.c_int * 5)(*x_ndhwc), (C.c_int * 5)(*dy_ndhwc), n_pad, kc, split_k, sms,
+                                   *[C.byref(o) for o in out]))
+    return tuple(o.value for o in out)
+
+
+def conv_wgrad_forms():
+    """Every (32-row blocks per CTA, GEMM columns) form of conv_wgrad, in the order of its form indices."""
+    n = lib().vp_conv_wgrad_forms(None, None, 0)
+    blocks, bn = (C.c_int * n)(), (C.c_int * n)()
+    lib().vp_conv_wgrad_forms(blocks, bn, n)
+    return list(zip(blocks, bn))
+
+
 def eff_taps(k, kind):
     if kind == WKIND_POOLED:
         return (k[1] + 1) * (k[2] + 1)

@@ -68,10 +68,14 @@ class ConvLayer(object):
     """One convolution of the path (generator, posterior encoder and discriminator alike): reference-layout parameters +
     packed tensor-core weights.  `spec` is the ConcatSpec of the input buffer, or (ci_ref, ci_int, cmap) given directly
     (cmap None = identity).  `inv_scale` (optional device scalar, the spectral-norm sigma) divides the weights in every pack.
-    In the fp32-exact mode (`model.exact`) every call runs as three TF32 passes (conv3x) against the residual packs."""
+    In the fp32-exact mode (`model.exact`) every call runs as three TF32 passes (conv3x) against the residual packs.
+    `prefilled`: the forward's output already holds an addend when the layer runs (the dense term of a conditioning site
+    without tile-concat), which the epilogue adds before the bias and the activation."""
 
-    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co, inv_scale=None, gates=False):
+    def __init__(self, model, wname, bname, k, kind, stride, pad, transposed, spec, co, inv_scale=None, gates=False,
+                 prefilled=False):
         self.model, self.wname, self.bname = model, wname, bname
+        self.prefilled = prefilled
         self.k, self.kind, self.stride, self.pad, self.transposed = k, kind, stride, pad, transposed
         self.co, self.inv_scale = co, inv_scale
         self.ci_ref, self.ci_int, cmap = (spec.ref_channels, spec.cstride, spec.cmap) if isinstance(spec, ConcatSpec) else spec
@@ -119,25 +123,30 @@ class ConvLayer(object):
         ov = L.tensor_view(self._view(out), self.co if out_c is None else out_c, out_off)
         bias = self.model.params[self.bname] if self.bname else None
         if self.model.exact:
-            conv3x(x, self.ci_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, ov, bias, act, alpha)
+            conv3x(x, self.ci_int, self.geom, self.wp, self.wp_lo, self.n_pad, self.kc, ov, bias, act, alpha, self.prefilled)
+            return
+        if self.prefilled:      # out = act(out + conv + bias): needs an unsplit call
+            L.conv_igemm(xv, self.geom, self.wp, self.n_pad, self.kc, ov, bias, act, alpha, 1, 2)
             return
         L.conv_igemm(xv, self.geom, self.wp, self.n_pad, self.kc, ov, bias, act, alpha, split_k)
 
     def lstm_fwd(self, x, z, c_prev, c_new, h_dests):
         """One norm-free ConvLSTM step from the GATES packs: z = conv(x) + bias (natural gate order), c_new and h (to the
         (address, cstride) slices h_dests) from the engine's epilogue.  fp32-exact mode: two partial passes add into a
-        zeroed z, the third adds the residual-weight pass and runs the cell."""
+        zeroed z, the third adds the residual-weight pass and runs the cell.  A prefilled z keeps its addend: every pass
+        adds to it."""
         x = self._view(x)
         xv = L.tensor_view(x, self.ci_int)
         cell = (z, self.model.params[self.bname], c_prev, c_new, h_dests)
         if self.model.exact:
-            z.zero_()
+            if not self.prefilled:
+                z.zero_()
             L.conv_lstm_fwd(xv, self.geom, self.wp, self.n_pad, self.kc, *cell, accumulate=1)
             L.conv_lstm_fwd(L.tensor_view(L.tf32_residual(x), self.ci_int), self.geom, self.wp, self.n_pad, self.kc, *cell,
                             accumulate=1)
             L.conv_lstm_fwd(xv, self.geom, self.wp_lo, self.n_pad, self.kc, *cell, accumulate=2)
             return
-        L.conv_lstm_fwd(xv, self.geom, self.wp, self.n_pad, self.kc, *cell)
+        L.conv_lstm_fwd(xv, self.geom, self.wp, self.n_pad, self.kc, *cell, accumulate=2 if self.prefilled else 0)
 
     def dgrad(self, dy, dx, dy_c=None, accumulate=False, act_y=None, addend=None, act=L.ACT_NONE, alpha=0.0):
         """dx[.., ci_int] (+)= conv^T(dy): the same engine with the transposed flag flipped.  With act_y, the output of the
@@ -262,8 +271,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             if getattr(hp, key + '_layer') not in table:      # ops.get_*_layer (ops.py:1052-1098)
                 raise ValueError('Invalid %s layer %s' % (key, getattr(hp, key + '_layer')))
         unsupported = []
-        for key, want in (('where_add', 'all'), ('use_tile_concat', True),
-                          ('conv_rnn', 'lstm'), ('use_e_rnn', False), ('learn_prior', False),
+        for key, want in (('conv_rnn', 'lstm'), ('use_e_rnn', False), ('learn_prior', False),
                           ('joint_gan_optimization', False), ('use_same_discriminator', False)):
             # (`repeat` is accepted with any value: train.py sets it to the dataset's time_shift (train.py:160) and no model
             #  code of the reference reads it, base_model.py:90-95)
@@ -351,6 +359,31 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         """The activation of the generator's norm_layer sites (activation_layer)."""
         return ACTIVATIONS[self.hparams.activation_layer]
 
+    def _zsite(self, li, rnn=False):
+        """How the conditioning vector state_action_z = [actions | state | rnn_z] reaches a site of generator layer li
+        (savp_model.py:456-518): the h{li} convolution (rnn=False) or the layer's ConvLSTM / conv_h site (rnn=True).
+        'tile' (use_tile_concat): tiled over space as extra input channels of the convolution; 'dense': the convolution reads
+        the spatial input alone and dense(v) is added to its output before the norm (_maybe_tile_concat_layer, :983-993;
+        the ConvLSTM's `weights`, rnn_ops.py:128-146); None: the site does not see the vector.  where_add='all' feeds every
+        site, 'input' h0 alone, 'middle' the first decoder layer alone."""
+        hp = self.hparams
+        if rnn:
+            takes = hp.where_add == 'all'
+        else:
+            takes = hp.where_add == 'all' or li == {'input': 0, 'middle': len(self.enc_specs)}[hp.where_add]
+        if not takes:
+            return None
+        return 'tile' if hp.use_tile_concat else 'dense'
+
+    def _zdense_name(self, li, rnn=False):
+        """The [Zc, site channels] kernel of the dense term of a 'dense' site (no bias)."""
+        sc = 'generator/rnn/savp_cell'
+        if not rnn:
+            return '%s/h%d/dense/kernel' % (sc, li)
+        if self.hparams.ablation_rnn:
+            return '%s/conv_h%d/dense/kernel' % (sc, li)
+        return '%s/lstm_h%d/basic_conv2dlstm_cell/weights' % (sc, li)
+
     def _hconv_layer(self, li, cin, oc):
         """(scope, kernel shape, weight kind, kernel size, pad before, transposed) of the h{li} convolution with cin input
         channels (tile-concat included)."""
@@ -428,27 +461,39 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             if self.norm_scope:
                 norm('%s/%s' % (site, self.norm_scope), c)
 
+        def tile(i, rnn=False):     # the tile-concat channels of a site's input
+            return Zc if self._zsite(i, rnn) == 'tile' else 0
+
+        def zdense(i, c, rnn=False):
+            # created after the site's convolution and before its norm, as the reference does; [0, c] without a vector
+            if self._zsite(i, rnn) == 'dense':
+                specs[self._zdense_name(i, rnn)] = ((Zc, c), 'kernel')
+
         def lstm(i, cin, oc):
+            zc = tile(i, rnn=True)
             if hp.ablation_rnn:     # conv 5x5 + norm_layer + activation_layer, no state (savp_model.py:472-475)
-                specs['%s/conv_h%d/conv2d/kernel' % (sc, i)] = ((5, 5, cin + Zc, oc), 'kernel')
+                specs['%s/conv_h%d/conv2d/kernel' % (sc, i)] = ((5, 5, cin + zc, oc), 'kernel')
                 specs['%s/conv_h%d/conv2d/bias' % (sc, i)] = ((oc,), 'zeros')
+                zdense(i, oc, rnn=True)
                 site_norm('%s/conv_h%d' % (sc, i), oc)
                 return
             b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, i)
-            specs[b + '/kernel'] = ((5, 5, cin + Zc + oc, 4 * oc), 'kernel')
+            specs[b + '/kernel'] = ((5, 5, cin + zc + oc, 4 * oc), 'kernel')
+            if not self.cell_norm:      # norm-free cell: the gate convolution has a bias (rnn_ops.py:122-125)
+                specs[b + '/bias'] = ((4 * oc,), 'zeros')
+            zdense(i, 4 * oc, rnn=True)
             if self.cell_norm:
                 norm(b + '/input_transform_forget_output', 4 * oc)
                 norm(b + '/state', oc)
-            else:       # norm-free cell: the gate convolution has a bias (rnn_ops.py:122-125)
-                specs[b + '/bias'] = ((4 * oc,), 'zeros')
-                if hp.ablation_conv_rnn_norm:      # instance norm of the cell output h (savp_model.py:380-383)
-                    norm('%s/lstm_h%d/InstanceNorm' % (sc, i), oc)
+            elif hp.ablation_conv_rnn_norm:      # instance norm of the cell output h (savp_model.py:380-383)
+                norm('%s/lstm_h%d/InstanceNorm' % (sc, i), oc)
         outs = []
         cin = 2 * C
         for i, (oc, use) in enumerate(enc):
-            scope, shape = self._hconv_layer(i, cin + Zc, oc)[:2]
+            scope, shape = self._hconv_layer(i, cin + tile(i), oc)[:2]
             specs[scope + '/kernel'] = (shape, 'kernel')
             specs[scope + '/bias'] = ((oc,), 'zeros')
+            zdense(i, oc)
             site_norm('%s/h%d' % (sc, i), oc)
             if use:
                 lstm(i, oc, oc)
@@ -458,9 +503,10 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         for i, (oc, use) in enumerate(dec):
             li = n_enc + i
             cin = outs[-1] if i == 0 else outs[-1] + outs[n_enc - i - 1]
-            scope, shape = self._hconv_layer(li, cin + Zc, oc)[:2]
+            scope, shape = self._hconv_layer(li, cin + tile(li), oc)[:2]
             specs[scope + '/kernel'] = (shape, 'kernel')
             specs[scope + '/bias'] = ((oc,), 'zeros')
+            zdense(li, oc)
             site_norm('%s/h%d' % (sc, li), oc)
             if use:
                 lstm(li, oc, oc)
@@ -862,7 +908,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         self.convs = []
         self.Bf = {}   # name -> stacked buffer
         Bf = self.Bf
-        zseg = [('z', Zc)] if Zc else []
+        # the use_tile_concat=False sites (dense kernel, output buffer, channel offset, channels, gradient buffer): dense(v)
+        # is broadcast into the convolution's output before it runs, for every step at once (_broadcast_z)
+        self.zdense = []
         self.gl = []   # per generator layer dict
         res = [(H >> (i + 1), W >> (i + 1)) for i in range(n_enc)]
         for i in range(len(dec)):
@@ -874,39 +922,43 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             hh, ww = res[li]
             ih, iw = (H, W) if li == 0 else res[li - 1]
             d = dict(li=li, oc=oc, use=use, h=hh, w=ww, is_enc=is_enc)
+            d['zin'], d['zr'] = self._zsite(li), (self._zsite(li, rnn=True) if use else None)
+            zseg = [('z', Zc)] if (Zc and d['zin'] == 'tile') else []
+            rzseg = [('z', Zc)] if (Zc and d['zr'] == 'tile') else []
             if li == 0:
-                segs = [('image', C), ('first', C)] + zseg
+                segs = [('image', C), ('first', C)]
             elif is_enc or li == n_enc:
-                segs = [('x', outs[-1])] + zseg
+                segs = [('x', outs[-1])]
             else:
-                segs = [('x', outs[-1]), ('skip', outs[n_enc - (li - n_enc) - 1])] + zseg
-            d['in_spec'] = ConcatSpec(segs)
+                segs = [('x', outs[-1]), ('skip', outs[n_enc - (li - n_enc) - 1])]
+            d['in_spec'] = ConcatSpec(segs + zseg)
             Bf['in%d' % li] = self._z(S, NB, ih, iw, d['in_spec'].cstride)
             scope, _, kind, ks, pb, transposed = self._hconv_layer(li, d['in_spec'].ref_channels, oc)
             d['conv'] = ConvLayer(self, scope + '/kernel', scope + '/bias', (1, ks, ks), kind, (1, 2, 2), (0, pb, pb), transposed,
-                                  d['in_spec'], oc)
+                                  d['in_spec'], oc, prefilled=bool(Zc) and d['zin'] == 'dense')
             self.convs.append(d['conv'])
             Bf['pre%d' % li] = self._z(S, NB, hh, ww, oc)
             Bf['nst%d' % li] = self._norm_stats(S, NB, oc)
             if use and hp.ablation_rnn:
                 # the stateless conv_h{li} site on (h{li} | z): conv -> rpre -> norm + activation -> out
-                d['rin_spec'] = ConcatSpec([('x', oc)] + zseg)
+                d['rin_spec'] = ConcatSpec([('x', oc)] + rzseg)
                 Bf['rin%d' % li] = self._z(S, NB, hh, ww, d['rin_spec'].cstride)
                 s = '%s/conv_h%d' % (sc, li)
                 d['rconv'] = ConvLayer(self, s + '/conv2d/kernel', s + '/conv2d/bias', (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
-                                       (0, 2, 2), False, d['rin_spec'], oc)
+                                       (0, 2, 2), False, d['rin_spec'], oc, prefilled=bool(Zc) and d['zr'] == 'dense')
                 d['rname'] = s
                 self.convs.append(d['rconv'])
                 Bf['rpre%d' % li] = self._z(S, NB, hh, ww, oc)
                 Bf['rnst%d' % li] = self._norm_stats(S, NB, oc)
                 Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
             elif use:
-                d['rin_spec'] = ConcatSpec([('x', oc)] + zseg + [('h', oc)])
+                d['rin_spec'] = ConcatSpec([('x', oc)] + rzseg + [('h', oc)])
                 Bf['rin%d' % li] = self._z(S + 1, NB, hh, ww, d['rin_spec'].cstride)
                 b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, li)
                 plain = not self.cell_norm
                 d['rconv'] = ConvLayer(self, b + '/kernel', b + '/bias' if plain else None, (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
-                                       (0, 2, 2), False, d['rin_spec'], 4 * oc, gates=plain)
+                                       (0, 2, 2), False, d['rin_spec'], 4 * oc, gates=plain,
+                                       prefilled=bool(Zc) and d['zr'] == 'dense')
                 d['rname'] = b
                 self.convs.append(d['rconv'])
                 Bf['gpre%d' % li] = self._z(S, NB, hh, ww, 4 * oc)
@@ -922,6 +974,17 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                     Bf['hst%d' % li] = self._z(S, NB, oc, 2)
             else:
                 Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
+            # where each convolution of the layer writes its output (before the norm; the activation for norm_layer='none')
+            none = hp.norm_layer == 'none'
+            if d['conv'].prefilled:
+                dst = (Bf['rin%d' % li], d['rin_spec'].off('x')) if use else (Bf['out%d' % li], 0)
+                self.zdense.append((self._zdense_name(li), *(dst if none else (Bf['pre%d' % li], 0)), oc, 'dpre%d' % li))
+            if use and d['rconv'].prefilled:
+                if hp.ablation_rnn:
+                    self.zdense.append((self._zdense_name(li, True), Bf[('out%d' if none else 'rpre%d') % li], 0, oc,
+                                        'drpre%d' % li))
+                else:
+                    self.zdense.append((self._zdense_name(li, True), Bf['gpre%d' % li], 0, 4 * oc, 'dgpre%d' % li))
             outs.append(oc)
             self.gl.append(d)
         nl = len(self.gl)
@@ -995,6 +1058,8 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                 Bf['ppix'] = self._z(S, NB, H, W, Dp)
         if Zc:
             Bf['zvec'] = self._z(S, NB, _ceil4(Zc))
+        if self.zdense:      # dense(v) of one site at a time, [S * NB, site channels]
+            Bf['zw'] = self._z(S * NB, max(s[3] for s in self.zdense))
         if self.Sd:
             Bf['states'] = self._z(S, NB, self.Sd)     # ground-truth states of both unrolls
             Bf['gstates'] = self._z(S, NB, self.Sd)    # predicted states (savp_model.py:655-658)
@@ -1322,13 +1387,19 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             li = d['li']
             buf = Bf['in%d' % li]
             sp = d['in_spec']
-            L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * sp.off('z'), sp.cstride, S * NB,
-                                 buf.shape[2] * buf.shape[3], Zc)
-            if d['use']:
+            if d['zin'] == 'tile':
+                L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * sp.off('z'), sp.cstride, S * NB,
+                                     buf.shape[2] * buf.shape[3], Zc)
+            if d['zr'] == 'tile':
                 buf = Bf['rin%d' % li]
                 sp = d['rin_spec']
                 L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * sp.off('z'), sp.cstride, S * NB,
                                      buf.shape[2] * buf.shape[3], Zc)
+        # the sites without tile-concat: their convolution's output starts as dense(v) of its step and row, and the
+        # convolution adds to it (ConvLayer.prefilled)
+        for name, buf, off, c, _ in self.zdense:
+            L.dense_fwd(Bf['zvec'], Zp, self.params[name], None, Bf['zw'], c, S * NB, Zc, c)
+            L.broadcast_channels(Bf['zw'], c, buf.data_ptr() + 4 * off, buf.shape[-1], S * NB, buf.shape[-2] * buf.shape[-3], c)
 
     def _h_dests(self, li, t):
         """Where the output of generator layer li at step t must land (its consumers' concat slices)."""

@@ -263,6 +263,8 @@ class TrainMixin(object):
             G['dfpre'] = z(S, NB, H, W, ngf)
         if self.Zc:
             G['dzvec'] = torch.zeros_like(Bf['zvec'])
+        if self.zdense:     # per-row sums of a dense site's output gradient
+            G['dzw'] = torch.zeros_like(Bf['zw'])
         if hp.nz:
             nz = hp.nz
             if self.z_cell in ('lstm', 'gru'):
@@ -501,8 +503,14 @@ class TrainMixin(object):
         sc_cell = 'generator/rnn/savp_cell'
         if hp.learn_initial_state:
             self._initial_state_grads(conv=True)
+        if self.Zc:
+            G['dzvec'].zero_()
+        zdense = {s[4]: s for s in self.zdense}
         for d in self.gl:
             li = d['li']
+            for key in ('dpre%d' % li, 'drpre%d' % li, 'dgpre%d' % li):
+                if key in zdense:
+                    self._zdense_backward(*zdense[key])
             d['conv'].wgrad(Bf['in%d' % li], G['dpre%d' % li])
             L.colsum(G['dpre%d' % li].data_ptr(), d['oc'], Gp[d['conv'].bname], 1, S * NB * d['h'] * d['w'], d['oc'])
             if d['use']:
@@ -544,11 +552,10 @@ class TrainMixin(object):
             return
         # tile_concat adjoint: sum the z-slot gradients of every concat buffer over space
         Zc, Zp = self.Zc, _ceil4(self.Zc)
-        G['dzvec'].zero_()
         for d in self.gl:
             li = d['li']
-            for key, spn in (('din%d' % li, 'in_spec'), ('drin%d' % li, 'rin_spec')):
-                if spn == 'rin_spec' and not d['use']:
+            for key, spn, form in (('din%d' % li, 'in_spec', d['zin']), ('drin%d' % li, 'rin_spec', d['zr'])):
+                if form != 'tile':
                     continue
                 buf = G[key][:S]
                 sp = d[spn]
@@ -619,6 +626,18 @@ class TrainMixin(object):
                 x_in = Bf['pairs']
             el['conv'].wgrad(x_in, G['depre%d' % i])
             L.colsum(G['depre%d' % i].data_ptr(), oc, Gp[el['conv'].bname], 1, S * B * pos, oc)
+
+    def _zdense_backward(self, name, buf, off, c, dy):
+        """The dense term of a site without tile-concat (out = conv(h) + dense(v, W)): its output gradient summed over space
+        per step and row, then dW += v^T sum and dv (into dzvec, the gradient the tile-concat sites' z slots give) += sum W^T.
+        For a ConvLSTM, dy is the gates' pre-activation gradient in the natural gate order."""
+        G, P = self.Gb, self.params
+        S, NB, Zc, Zp = self.S, self.NB, self.Zc, _ceil4(self.Zc)
+        g = G[dy]
+        G['dzw'].zero_()
+        L.colsum(g.data_ptr(), c, G['dzw'], S * NB, g.shape[-2] * g.shape[-3], c)
+        L.dense_bwd(self.Bf['zvec'], Zp, P[name], G['dzw'], c, S * NB, Zc, c, dx=G['dzvec'], dx_stride=Zp, dx_accumulate=True,
+                    dw=self.grads[name])
 
     def _initial_state_grads(self, conv):
         """Gradients of the learned initial states: the sum over the NB rows of the t = 0 state gradient -- dc[0] and the h

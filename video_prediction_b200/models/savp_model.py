@@ -191,6 +191,82 @@ def conv3x(x, c, geom, wp, wp_lo, n_pad, kc, ov, bias, act, alpha, accumulate=Fa
         L.conv_igemm_actgrad(xv, geom, wp_lo, n_pad, kc, ov, aux[0], aux[1], aux[2], alpha, accumulate=2)
 
 
+class NormSite(object):
+    """One conv -> norm_layer -> activation site (ops.get_norm_layer, ops.py:1062-1073): h{i}, conv_h{i}, the h_flow /
+    h_scratch / h_masks heads and posterior encoder layers 2 and up.  'instance' and 'layer' run the convolution into the `pre`
+    buffer and the norm kernel from there into the output slice; 'none' has the convolution's epilogue apply bias +
+    activation straight into that slice, and the backward takes the activation gradient from the output.
+
+    Buffers are Bf keys (x: the convolution's input, read by the weight gradient; out: the output slice at channel out_off),
+    their gradients the Gb key 'd' + pre.  They are indexed by step, and t=None is the whole buffer (the posterior encoder
+    runs every step at once); `rows` = samples per call.  A prefilled convolution (a conditioning site without tile-concat)
+    has its dense term (kernel `zname`) in `zdense`: (kernel, buffer, channel offset, channels, Gb key of its gradient)."""
+
+    def __init__(self, model, conv, scope, x, pre, stats, out, out_off, rows, act, alpha=0.0, zname=None):
+        self.model, self.conv, self.scope = model, conv, scope
+        self.x, self.pre, self.dpre, self.stats, self.out, self.out_off = x, pre, 'd' + pre, stats, out, out_off
+        pb = model.Bf[pre]
+        self.rows, self.positions, self.c = rows, pb.shape[-3] * pb.shape[-2], conv.co
+        self.out_cs = model.Bf[out].shape[-1]
+        self.act, self.alpha = act, alpha
+        self.norm = model.norm_scope and '%s/%s' % (scope, model.norm_scope)      # variable scope, None for 'none'
+        self.zdense = None
+        if conv.prefilled:      # the dense term lands where the convolution writes
+            self.zdense = (zname,) + ((model.Bf[out], out_off) if self.norm is None else (pb, 0)) + (self.c, self.dpre)
+
+    @staticmethod
+    def _at(bufs, key, t):
+        return bufs[key] if t is None else bufs[key][t]
+
+    def _out(self, t):
+        return self._at(self.model.Bf, self.out, t).data_ptr() + 4 * self.out_off
+
+    def conv_fwd(self, x, t):
+        """The convolution of step t on its input x."""
+        if self.norm is None:
+            self.conv.fwd(x, self._at(self.model.Bf, self.out, t), out_off=self.out_off, act=self.act, alpha=self.alpha)
+        else:
+            self.conv.fwd(x, self._at(self.model.Bf, self.pre, t))
+
+    def norm_fwd(self, t):
+        """out = act(norm(pre)) of step t; nothing to do for 'none'."""
+        if self.norm is None:
+            return
+        m, c = self.model, self.c
+        fn = L.inorm_act if m.hparams.norm_layer == 'instance' else L.lnorm_act
+        fn(self._at(m.Bf, self.pre, t).data_ptr(), c, self._out(t), self.out_cs, self.rows, self.positions, c,
+           m.params[self.norm + '/gamma'], m.params[self.norm + '/beta'], self.act, self.alpha, self._at(m.Bf, self.stats, t))
+
+    def bwd(self, t, srcs, dx, accumulate=False):
+        """dpre of step t from the gradient sources `srcs` [(address, cstride)] of the output, summed in that order
+        (accumulating the norm's gamma / beta gradients), then dx (+)= conv^T(dpre)."""
+        m, c = self.model, self.c
+        dpre = self._at(m.Gb, self.dpre, t)
+        dp = dpre.data_ptr()
+        if self.norm is None:
+            rows = self.rows * self.positions
+            if len(srcs) > 2:            # act_bwd adds two sources: fold the others into dpre first
+                L.axpy_channels(srcs[0][0], srcs[0][1], dp, c, rows, c, accumulate=False)
+                for a, cs in srcs[1:-1]:
+                    L.axpy_channels(a, cs, dp, c, rows, c)
+                srcs = [(dp, c), srcs[-1]]
+            b = srcs[1] if len(srcs) > 1 else (0, c)
+            L.act_bwd(self._out(t), self.out_cs, srcs[0][0], srcs[0][1], b[0], b[1], dp, c, rows, c, self.act, self.alpha)
+        else:
+            fn = L.inorm_act_bwd if m.hparams.norm_layer == 'instance' else L.lnorm_act_bwd
+            P, Gp, nm = m.params, m.grads, self.norm
+            fn(self._at(m.Bf, self.pre, t).data_ptr(), c, srcs, dp, c, self.rows, self.positions, c, P[nm + '/gamma'],
+               P[nm + '/beta'], self._at(m.Bf, self.stats, t), self.act, self.alpha, Gp[nm + '/gamma'], Gp[nm + '/beta'])
+        self.conv.dgrad(dpre, dx, accumulate=accumulate)
+
+    def param_grads(self):
+        """The weight gradient over every step (one GEMM), then the bias gradient."""
+        m = self.model
+        dy = m.Gb[self.dpre]
+        self.conv.wgrad(m.Bf[self.x], dy)
+        L.colsum(dy.data_ptr(), self.c, m.grads[self.conv.bname], 1, dy.numel() // self.c, self.c)
+
+
 # The generator's h{i} convolutions (savp_model.py:394-397, 461-464, 494-500; ops.get_downsample_layer /
 # get_upsample_layer, ops.py:1077-1098): name -> (variable scope, weight kind, pad before, transposed), all with stride 2.
 # The kernel is [k, k, cin, oc] -- deconv2d's is [3, 3, oc, cin], conv2d_transpose's filter layout.
@@ -418,13 +494,53 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             raise NotImplementedError
         return enc, dec
 
+    def _generator_plan(self):
+        """The generator's layers from the hparams and shapes alone (no device): per layer li its oc, use (ConvLSTM after
+        the h{li} site), output and input extents h, w / ih, iw, zin / zr (_zsite of the h{li} and the recurrent site),
+        in_spec (the h{li} input: image | first image, or x | skip, then z when tile-concatenated), hconv (_hconv_layer)
+        and, with use, the recurrent site: rin_spec (x | z for conv_h{li}, x | z | h for the ConvLSTM), its scope rname,
+        its kernel / bias names and its output channels rco."""
+        hp = self.hparams
+        sc = 'generator/rnn/savp_cell'
+        n_enc = len(self.enc_specs)
+        plan = []
+        h, w = self.H, self.W
+
+        def zseg(form):     # the z segment of a site's input when it tile-concatenates the vector
+            return [('z', self.Zc)] if (self.Zc and form == 'tile') else []
+        for li, (oc, use) in enumerate(self.enc_specs + self.dec_specs):
+            is_enc = li < n_enc
+            d = dict(li=li, oc=oc, use=use, is_enc=is_enc, ih=h, iw=w, zin=self._zsite(li),
+                     zr=self._zsite(li, rnn=True) if use else None)
+            h, w = (h // 2, w // 2) if is_enc else (h * 2, w * 2)
+            d['h'], d['w'] = h, w
+            if li == 0:
+                segs = [('image', self.C), ('first', self.C)]
+            elif is_enc or li == n_enc:
+                segs = [('x', plan[-1]['oc'])]
+            else:       # skip connection: decoder layer n_enc + i reads layer n_enc - i - 1
+                segs = [('x', plan[-1]['oc']), ('skip', plan[2 * n_enc - li - 1]['oc'])]
+            d['in_spec'] = ConcatSpec(segs + zseg(d['zin']))
+            d['hconv'] = self._hconv_layer(li, d['in_spec'].ref_channels, oc)
+            if use:
+                if hp.ablation_rnn:     # the stateless conv_h{li} site (savp_model.py:472-475)
+                    d['rname'] = '%s/conv_h%d' % (sc, li)
+                    d['rin_spec'] = ConcatSpec([('x', oc)] + zseg(d['zr']))
+                    d['rkernel'], d['rbias'], d['rco'] = d['rname'] + '/conv2d/kernel', d['rname'] + '/conv2d/bias', oc
+                else:                   # the norm-free cell's gate convolution has a bias (rnn_ops.py:122-125)
+                    d['rname'] = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, li)
+                    d['rin_spec'] = ConcatSpec([('x', oc)] + zseg(d['zr']) + [('h', oc)])
+                    d['rkernel'], d['rco'] = d['rname'] + '/kernel', 4 * oc
+                    d['rbias'] = None if self.cell_norm else d['rname'] + '/bias'
+            plan.append(d)
+        return plan
+
     def _generator_param_specs(self):
         """name -> (shape, init) with the reference's variable scopes (generator/...)."""
         hp = self.hparams
-        H, W, C, A = self.H, self.W, self.C, self.A
+        C, A = self.C, self.A
         specs = OrderedDict()
         Zc = self.Zc
-        enc, dec = self.enc_specs, self.dec_specs
         if hp.nz:
             sc = 'generator/encoder'
             cin = 2 * C + A
@@ -461,63 +577,37 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             if self.norm_scope:
                 norm('%s/%s' % (site, self.norm_scope), c)
 
-        def tile(i, rnn=False):     # the tile-concat channels of a site's input
-            return Zc if self._zsite(i, rnn) == 'tile' else 0
-
-        def zdense(i, c, rnn=False):
+        def zdense(d, c, rnn=False):
             # created after the site's convolution and before its norm, as the reference does; [0, c] without a vector
-            if self._zsite(i, rnn) == 'dense':
-                specs[self._zdense_name(i, rnn)] = ((Zc, c), 'kernel')
-
-        def lstm(i, cin, oc):
-            zc = tile(i, rnn=True)
-            if hp.ablation_rnn:     # conv 5x5 + norm_layer + activation_layer, no state (savp_model.py:472-475)
-                specs['%s/conv_h%d/conv2d/kernel' % (sc, i)] = ((5, 5, cin + zc, oc), 'kernel')
-                specs['%s/conv_h%d/conv2d/bias' % (sc, i)] = ((oc,), 'zeros')
-                zdense(i, oc, rnn=True)
-                site_norm('%s/conv_h%d' % (sc, i), oc)
-                return
-            b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, i)
-            specs[b + '/kernel'] = ((5, 5, cin + zc + oc, 4 * oc), 'kernel')
-            if not self.cell_norm:      # norm-free cell: the gate convolution has a bias (rnn_ops.py:122-125)
-                specs[b + '/bias'] = ((4 * oc,), 'zeros')
-            zdense(i, 4 * oc, rnn=True)
-            if self.cell_norm:
-                norm(b + '/input_transform_forget_output', 4 * oc)
-                norm(b + '/state', oc)
-            elif hp.ablation_conv_rnn_norm:      # instance norm of the cell output h (savp_model.py:380-383)
-                norm('%s/lstm_h%d/InstanceNorm' % (sc, i), oc)
-        outs = []
-        cin = 2 * C
-        for i, (oc, use) in enumerate(enc):
-            scope, shape = self._hconv_layer(i, cin + tile(i), oc)[:2]
+            if d['zr' if rnn else 'zin'] == 'dense':
+                specs[self._zdense_name(d['li'], rnn)] = ((Zc, c), 'kernel')
+        plan = self._generator_plan()
+        for d in plan:
+            li, oc = d['li'], d['oc']
+            scope, shape = d['hconv'][:2]
             specs[scope + '/kernel'] = (shape, 'kernel')
             specs[scope + '/bias'] = ((oc,), 'zeros')
-            zdense(i, oc)
-            site_norm('%s/h%d' % (sc, i), oc)
-            if use:
-                lstm(i, oc, oc)
-            outs.append(oc)
-            cin = oc
-        n_enc = len(enc)
-        for i, (oc, use) in enumerate(dec):
-            li = n_enc + i
-            cin = outs[-1] if i == 0 else outs[-1] + outs[n_enc - i - 1]
-            scope, shape = self._hconv_layer(li, cin + tile(li), oc)[:2]
-            specs[scope + '/kernel'] = (shape, 'kernel')
-            specs[scope + '/bias'] = ((oc,), 'zeros')
-            zdense(li, oc)
+            zdense(d, oc)
             site_norm('%s/h%d' % (sc, li), oc)
-            if use:
-                lstm(li, oc, oc)
-            outs.append(oc)
-        nl = n_enc + len(dec)
+            if not d['use']:
+                continue
+            specs[d['rkernel']] = ((5, 5, d['rin_spec'].ref_channels, d['rco']), 'kernel')
+            if d['rbias']:
+                specs[d['rbias']] = ((d['rco'],), 'zeros')
+            zdense(d, d['rco'], rnn=True)
+            if hp.ablation_rnn:     # conv 5x5 + norm_layer + activation_layer, no state
+                site_norm(d['rname'], oc)
+            elif self.cell_norm:
+                norm(d['rname'] + '/input_transform_forget_output', 4 * oc)
+                norm(d['rname'] + '/state', oc)
+            elif hp.ablation_conv_rnn_norm:      # instance norm of the cell output h (savp_model.py:380-383)
+                norm('%s/lstm_h%d/InstanceNorm' % (sc, li), oc)
+        nl = len(plan)
         kh, kw = hp.kernel_size
         comp = self.compositing(hp)
         nk, nlayers = comp['nk'], comp['L']
-        sh = H // (2 ** n_enc)
-        sw = W // (2 ** n_enc)
-        top = outs[-1]
+        small = plan[len(self.enc_specs) - 1]
+        top = plan[-1]['oc']
         if nk and hp.transformation == 'flow':     # savp_model.py:522-530: flow heads instead of the CDNA kernel dense layer
             specs['%s/h%d_flow/conv2d/kernel' % (sc, nl)] = ((3, 3, top, hp.ngf), 'kernel')
             specs['%s/h%d_flow/conv2d/bias' % (sc, nl)] = ((hp.ngf,), 'zeros')
@@ -525,7 +615,7 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             specs[sc + '/flows/conv2d/kernel'] = ((3, 3, hp.ngf, 2 * nk), 'kernel')
             specs[sc + '/flows/conv2d/bias'] = ((2 * nk,), 'zeros')
         elif nk:
-            specs[sc + '/cdna_kernels/dense/kernel'] = ((sh * sw * outs[n_enc - 1], kh * kw * nk), 'kernel')
+            specs[sc + '/cdna_kernels/dense/kernel'] = ((small['h'] * small['w'] * small['oc'], kh * kw * nk), 'kernel')
             specs[sc + '/cdna_kernels/dense/bias'] = ((kh * kw * nk,), 'zeros')
         heads = (['h%d_scratch' % nl] if comp['scratch'] else []) + (['h%d_masks' % nl] if nlayers > 1 else [])
         for nm in heads:
@@ -555,11 +645,9 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             return []
         leaves = []
         if not hp.ablation_rnn:
-            hh, ww = self.H, self.W
-            for li, (oc, use) in enumerate(self.enc_specs + self.dec_specs):
-                hh, ww = (hh // 2, ww // 2) if li < len(self.enc_specs) else (hh * 2, ww * 2)
-                if use:
-                    leaves += [((hh, ww, oc), 'c', li), ((hh, ww, oc), 'h', li)]
+            for d in self._generator_plan():
+                if d['use']:
+                    leaves += [((d['h'], d['w'], d['oc']), what, d['li']) for what in ('c', 'h')]
         if self.z_cell in ('lstm', 'gru'):
             leaves += [((hp.nz,), 'zc', -1)] if self.z_cell == 'lstm' else []
             leaves.append(((hp.nz,), 'zh', -1))
@@ -856,113 +944,60 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
     def _z(self, *shape):
         return torch.zeros(*shape, device=self.device, dtype=torch.float32)
 
-    # ------------------------------------------------------------------ norm_layer sites (ops.get_norm_layer, ops.py:1062-1073)
-    # Each site is conv -> normaliser -> activation.  'instance' and 'layer' run the convolution into a `pre` buffer and
-    # the norm kernel from there into the site's output slice; 'none' has the convolution's epilogue apply bias +
-    # activation straight into that slice, and the backward takes the activation gradient from the output.
     def _norm_stats(self, *lead_and_c):
-        """Per-call statistics of a site: [.., c, 2] (instance), [.., 2] (layer) or empty (none)."""
+        """Per-call statistics of a NormSite: [.., c, 2] (instance), [.., 2] (layer) or empty (none)."""
         lead, c = lead_and_c[:-1], lead_and_c[-1]
         return self._z(*lead, *{'instance': (c, 2), 'layer': (2,)}.get(self.hparams.norm_layer, (0,)))
-
-    def _site_conv(self, conv, x, pre, out, out_off=0, act=L.ACT_RELU, alpha=0.0):
-        if self.hparams.norm_layer == 'none':
-            conv.fwd(x, out, out_off=out_off, act=act, alpha=alpha)
-        else:
-            conv.fwd(x, pre)
-
-    def _site_norm(self, site, pre, out_addr, out_cs, n, positions, c, act, alpha, stats):
-        """out = act(norm(pre)) with the variables `site`/<norm_scope>; nothing to do for 'none'."""
-        if self.norm_scope is None:
-            return
-        nm = '%s/%s' % (site, self.norm_scope)
-        fn = L.inorm_act if self.hparams.norm_layer == 'instance' else L.lnorm_act
-        fn(pre.data_ptr(), c, out_addr, out_cs, n, positions, c, self.params[nm + '/gamma'], self.params[nm + '/beta'], act, alpha,
-           stats)
-
-    def _site_norm_bwd(self, site, pre, y_addr, y_cs, srcs, dpre, n, positions, c, act, alpha, stats):
-        """dpre from the gradient sources `srcs` (summed) of the site's output y (at y_addr); accumulates the norm's
-        gamma / beta gradients."""
-        if self.norm_scope is None:
-            rows, dp = n * positions, dpre.data_ptr()
-            if len(srcs) > 2:            # act_bwd adds two sources: fold the others into dpre first
-                L.axpy_channels(srcs[0][0], srcs[0][1], dp, c, rows, c, accumulate=False)
-                for a, cs in srcs[1:-1]:
-                    L.axpy_channels(a, cs, dp, c, rows, c)
-                srcs = [(dp, c), srcs[-1]]
-            b = srcs[1] if len(srcs) > 1 else (0, c)
-            L.act_bwd(y_addr, y_cs, srcs[0][0], srcs[0][1], b[0], b[1], dp, c, rows, c, act, alpha)
-            return
-        nm = '%s/%s' % (site, self.norm_scope)
-        fn = L.inorm_act_bwd if self.hparams.norm_layer == 'instance' else L.lnorm_act_bwd
-        P, Gp = self.params, self.grads
-        fn(pre.data_ptr(), c, srcs, dpre.data_ptr(), c, n, positions, c, P[nm + '/gamma'], P[nm + '/beta'], stats, act, alpha,
-           Gp[nm + '/gamma'], Gp[nm + '/beta'])
 
     def _build_generator(self):
         hp = self.hparams
         S, NB, H, W, C, Zc = self.S, self.NB, self.H, self.W, self.C, self.Zc
         sc = 'generator/rnn/savp_cell'
-        enc, dec = self.enc_specs, self.dec_specs
-        n_enc = len(enc)
+        n_enc = len(self.enc_specs)
+        act = self.site_act
         self.convs = []
         self.Bf = {}   # name -> stacked buffer
         Bf = self.Bf
-        # the use_tile_concat=False sites (dense kernel, output buffer, channel offset, channels, gradient buffer): dense(v)
-        # is broadcast into the convolution's output before it runs, for every step at once (_broadcast_z)
+        self.comp = comp = self.compositing(hp)
+        self.nk, self.nlayers = comp['nk'], comp['L']
+        self.kh, self.kw = hp.kernel_size
+        self.flow = hp.transformation == 'flow' and self.nk > 0      # the flow heads
+        self.cdna = hp.transformation == 'cdna' and self.nk > 0      # the CDNA kernel dense layer
+        # the use_tile_concat=False sites (NormSite.zdense entries, and the ConvLSTMs' gate buffers): dense(v) is broadcast
+        # into the convolution's output before it runs, for every step at once (_broadcast_z)
         self.zdense = []
-        self.gl = []   # per generator layer dict
-        res = [(H >> (i + 1), W >> (i + 1)) for i in range(n_enc)]
-        for i in range(len(dec)):
-            res.append((res[n_enc - 1][0] << (i + 1), res[n_enc - 1][1] << (i + 1)))
-        outs = []
-        for li in range(n_enc + len(dec)):
-            is_enc = li < n_enc
-            oc, use = enc[li] if is_enc else dec[li - n_enc]
-            hh, ww = res[li]
-            ih, iw = (H, W) if li == 0 else res[li - 1]
-            d = dict(li=li, oc=oc, use=use, h=hh, w=ww, is_enc=is_enc)
-            d['zin'], d['zr'] = self._zsite(li), (self._zsite(li, rnn=True) if use else None)
-            zseg = [('z', Zc)] if (Zc and d['zin'] == 'tile') else []
-            rzseg = [('z', Zc)] if (Zc and d['zr'] == 'tile') else []
-            if li == 0:
-                segs = [('image', C), ('first', C)]
-            elif is_enc or li == n_enc:
-                segs = [('x', outs[-1])]
-            else:
-                segs = [('x', outs[-1]), ('skip', outs[n_enc - (li - n_enc) - 1])]
-            d['in_spec'] = ConcatSpec(segs + zseg)
-            Bf['in%d' % li] = self._z(S, NB, ih, iw, d['in_spec'].cstride)
-            scope, _, kind, ks, pb, transposed = self._hconv_layer(li, d['in_spec'].ref_channels, oc)
+        # the z segments of the tile-concat inputs: zvec is broadcast into them (_broadcast_z), and their gradients are
+        # summed over space into dzvec
+        self.ztiles = []
+        self.gl = gl = self._generator_plan()
+        self.nl = nl = len(gl)
+
+        def slot(key, spec, seg):       # a segment of a concat buffer: (Bf key, Gb key, channel offset, cstride)
+            return key, 'd' + key, spec.off(seg), spec.cstride
+        for d in gl:
+            li, oc, use, hh, ww = d['li'], d['oc'], d['use'], d['h'], d['w']
+            sp, rsp = d['in_spec'], d.get('rin_spec')
+            Bf['in%d' % li] = self._z(S, NB, d['ih'], d['iw'], sp.cstride)
+            scope, _, kind, ks, pb, transposed = d['hconv']
             d['conv'] = ConvLayer(self, scope + '/kernel', scope + '/bias', (1, ks, ks), kind, (1, 2, 2), (0, pb, pb), transposed,
-                                  d['in_spec'], oc, prefilled=bool(Zc) and d['zin'] == 'dense')
+                                  sp, oc, prefilled=bool(Zc) and d['zin'] == 'dense')
             self.convs.append(d['conv'])
             Bf['pre%d' % li] = self._z(S, NB, hh, ww, oc)
             Bf['nst%d' % li] = self._norm_stats(S, NB, oc)
-            if use and hp.ablation_rnn:
-                # the stateless conv_h{li} site on (h{li} | z): conv -> rpre -> norm + activation -> out
-                d['rin_spec'] = ConcatSpec([('x', oc)] + rzseg)
-                Bf['rin%d' % li] = self._z(S, NB, hh, ww, d['rin_spec'].cstride)
-                s = '%s/conv_h%d' % (sc, li)
-                d['rconv'] = ConvLayer(self, s + '/conv2d/kernel', s + '/conv2d/bias', (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
-                                       (0, 2, 2), False, d['rin_spec'], oc, prefilled=bool(Zc) and d['zr'] == 'dense')
-                d['rname'] = s
+            if use:
+                # c[t], the h slot of rin[t]: the state entering step t of a ConvLSTM; conv_h{li} has no state
+                Bf['rin%d' % li] = self._z(S if hp.ablation_rnn else S + 1, NB, hh, ww, rsp.cstride)
+                d['rconv'] = ConvLayer(self, d['rkernel'], d['rbias'], (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1), (0, 2, 2), False,
+                                       rsp, d['rco'], gates=not (hp.ablation_rnn or self.cell_norm),
+                                       prefilled=bool(Zc) and d['zr'] == 'dense')
                 self.convs.append(d['rconv'])
+            if use and hp.ablation_rnn:
                 Bf['rpre%d' % li] = self._z(S, NB, hh, ww, oc)
                 Bf['rnst%d' % li] = self._norm_stats(S, NB, oc)
                 Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
             elif use:
-                d['rin_spec'] = ConcatSpec([('x', oc)] + rzseg + [('h', oc)])
-                Bf['rin%d' % li] = self._z(S + 1, NB, hh, ww, d['rin_spec'].cstride)
-                b = '%s/lstm_h%d/basic_conv2dlstm_cell' % (sc, li)
-                plain = not self.cell_norm
-                d['rconv'] = ConvLayer(self, b + '/kernel', b + '/bias' if plain else None, (1, 5, 5), L.WKIND_PLAIN, (1, 1, 1),
-                                       (0, 2, 2), False, d['rin_spec'], 4 * oc, gates=plain,
-                                       prefilled=bool(Zc) and d['zr'] == 'dense')
-                d['rname'] = b
-                self.convs.append(d['rconv'])
                 Bf['gpre%d' % li] = self._z(S, NB, hh, ww, 4 * oc)
-                Bf['c%d' % li] = self._z(S + 1, NB, hh, ww, oc)      # c[t] = state entering step t
+                Bf['c%d' % li] = self._z(S + 1, NB, hh, ww, oc)
                 if hp.learn_initial_state:
                     Bf['h0_%d' % li] = self._z(NB, hh, ww, oc)         # the learned h state tiled over the rows
                 if self.cell_norm:
@@ -972,48 +1007,65 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                     # IN(h): the layer's output, copied to its consumers; the raw h is the recurrent state only
                     Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
                     Bf['hst%d' % li] = self._z(S, NB, oc, 2)
+                d['rec'] = slot('rin%d' % li, rsp, 'h')
             else:
                 Bf['out%d' % li] = self._z(S, NB, hh, ww, oc)
-            # where each convolution of the layer writes its output (before the norm; the activation for norm_layer='none')
-            none = hp.norm_layer == 'none'
-            if d['conv'].prefilled:
-                dst = (Bf['rin%d' % li], d['rin_spec'].off('x')) if use else (Bf['out%d' % li], 0)
-                self.zdense.append((self._zdense_name(li), *(dst if none else (Bf['pre%d' % li], 0)), oc, 'dpre%d' % li))
-            if use and d['rconv'].prefilled:
-                if hp.ablation_rnn:
-                    self.zdense.append((self._zdense_name(li, True), Bf[('out%d' if none else 'rpre%d') % li], 0, oc,
-                                        'drpre%d' % li))
-                else:
-                    self.zdense.append((self._zdense_name(li, True), Bf['gpre%d' % li], 0, 4 * oc, 'dgpre%d' % li))
-            outs.append(oc)
-            self.gl.append(d)
-        nl = len(self.gl)
-        self.nl = nl
-        top = outs[-1]
-        kh, kw = hp.kernel_size
-        self.comp = comp = self.compositing(hp)
-        nk = comp['nk']
-        self.nk, self.kh, self.kw = nk, kh, kw
-        self.nlayers = comp['L']
-        self.flow = hp.transformation == 'flow' and nk > 0      # the flow heads
-        self.cdna = hp.transformation == 'cdna' and nk > 0      # the CDNA kernel dense layer
+            # the h{li} site writes the 'x' slot of the recurrent site's input, or the layer's own output
+            out = ('rin%d' % li, rsp.off('x')) if use else ('out%d' % li, 0)
+            d['site'] = NormSite(self, d['conv'], '%s/h%d' % (sc, li), 'in%d' % li, 'pre%d' % li, 'nst%d' % li, *out, NB, act,
+                                 zname=self._zdense_name(li))
+            zd = [d['site'].zdense]
+            if use and hp.ablation_rnn:
+                d['rsite'] = NormSite(self, d['rconv'], d['rname'], 'rin%d' % li, 'rpre%d' % li, 'rnst%d' % li, 'out%d' % li, 0,
+                                      NB, act, zname=self._zdense_name(li, rnn=True))
+                zd.append(d['rsite'].zdense)
+            elif use and d['rconv'].prefilled:
+                zd.append((self._zdense_name(li, rnn=True), Bf['gpre%d' % li], 0, 4 * oc, 'dgpre%d' % li))
+            d['zdense'] = [z for z in zd if z]
+            self.zdense += d['zdense']
+            for form, key, spec in ((d['zin'], 'in%d' % li, sp), (d['zr'], 'rin%d' % li, rsp)):
+                if Zc and form == 'tile':
+                    self.ztiles.append(slot(key, spec, 'z'))
+            # the consumers of the layer's output, in the order the forward writes them and the backward sums their
+            # gradients: the next layer's 'x' slot (after the top layer, the heads, which read its out buffer: no forward
+            # copy), the skip slot of decoder layer 2 n_enc - 1 - li, the CDNA kernel layer's flattened input.  A ConvLSTM
+            # also feeds its own h slot of step t + 1 (d['rec']): first in the forward, last in the backward.
+            d['wires'] = [slot('in%d' % (li + 1), gl[li + 1]['in_spec'], 'x') if li + 1 < nl else (None, 'dtop', 0, oc)]
+            if li < n_enc - 1:
+                j = 2 * n_enc - 1 - li
+                d['wires'].append(slot('in%d' % j, gl[j]['in_spec'], 'skip'))
+            if li == n_enc - 1 and self.cdna:
+                d['wires'].append(('small', 'dsmall', 0, oc))
         if self.cdna:
-            sl = self.gl[n_enc - 1]
+            sl = gl[n_enc - 1]
             Bf['small'] = self._z(S, NB, sl['h'] * sl['w'] * sl['oc'])
-            Bf['kraw'] = self._z(S, NB, kh * kw * nk)
-            Bf['kern'] = self._z(S, NB, kh * kw * nk)
-        top_spec = ConcatSpec([('x', top)])
-        self.top_spec = top_spec
-        hs_spec = ConcatSpec([('x', hp.ngf)])
+            Bf['kraw'] = self._z(S, NB, self.kh * self.kw * self.nk)
+            Bf['kern'] = self._z(S, NB, self.kh * self.kw * self.nk)
         # the masks-conv input: h_masks, then the L slots (the scratch image last)
         self.mk_spec = ConcatSpec([('hm', hp.ngf)] + [('l%d' % l, C) for l in range(self.nlayers)])
-        self.conv_scratch = self.conv_hmasks = self.conv_simg = self.conv_masks = None
-        if comp['scratch']:
-            self.conv_scratch = ConvLayer(self, '%s/h%d_scratch/conv2d/kernel' % (sc, nl), '%s/h%d_scratch/conv2d/bias' % (sc, nl),
-                                          (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
-        if self.nlayers > 1:
-            self.conv_hmasks = ConvLayer(self, '%s/h%d_masks/conv2d/kernel' % (sc, nl), '%s/h%d_masks/conv2d/bias' % (sc, nl),
-                                         (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
+        if self.flow:
+            Bf['fpre'] = self._z(S, NB, H, W, hp.ngf)
+            Bf['fst'] = self._norm_stats(S, NB, hp.ngf)
+            Bf['hf'] = self._z(S, NB, H, W, hp.ngf)
+            Bf['flows'] = self._z(S, NB, H, W, _ceil4(2 * self.nk))
+        Bf['spre'] = self._z(S, NB, H, W, hp.ngf)
+        Bf['mpre'] = self._z(S, NB, H, W, hp.ngf)
+        Bf['sst'] = self._norm_stats(S, NB, hp.ngf)
+        Bf['mst'] = self._norm_stats(S, NB, hp.ngf)
+        Bf['hs'] = self._z(S, NB, H, W, hp.ngf)
+        Bf['mk'] = self._z(S, NB, H, W, self.mk_spec.cstride)
+        top_spec = ConcatSpec([('x', gl[-1]['oc'])])
+        hs_spec = ConcatSpec([('x', hp.ngf)])
+
+        def head(nm, pre, stats, out, out_off=0):       # a 3x3 site on the top layer's output
+            conv = ConvLayer(self, '%s/%s/conv2d/kernel' % (sc, nm), '%s/%s/conv2d/bias' % (sc, nm), (1, 3, 3), L.WKIND_PLAIN,
+                             (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
+            return NormSite(self, conv, '%s/%s' % (sc, nm), 'out%d' % (nl - 1), pre, stats, out, out_off, NB, act)
+        self.scratch_site = head('h%d_scratch' % nl, 'spre', 'sst', 'hs') if comp['scratch'] else None
+        self.hmasks_site = head('h%d_masks' % nl, 'mpre', 'mst', 'mk', self.mk_spec.off('hm')) if self.nlayers > 1 else None
+        self.conv_scratch = self.scratch_site and self.scratch_site.conv
+        self.conv_hmasks = self.hmasks_site and self.hmasks_site.conv
+        self.conv_simg = self.conv_masks = None
         if comp['scratch']:
             self.conv_simg = ConvLayer(self, sc + '/scratch_image/conv2d/kernel', sc + '/scratch_image/conv2d/bias',
                                        (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, hs_spec, C)
@@ -1025,21 +1077,11 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                                         (1, 1, 1), (0, 1, 1), False, mspec, self.nlayers)
         self.convs += [c for c in (self.conv_scratch, self.conv_hmasks, self.conv_simg, self.conv_masks) if c is not None]
         if self.flow:
-            self.conv_hflow = ConvLayer(self, '%s/h%d_flow/conv2d/kernel' % (sc, nl), '%s/h%d_flow/conv2d/bias' % (sc, nl),
-                                        (1, 3, 3), L.WKIND_PLAIN, (1, 1, 1), (0, 1, 1), False, top_spec, hp.ngf)
+            self.hflow_site = head('h%d_flow' % nl, 'fpre', 'fst', 'hf')
+            self.conv_hflow = self.hflow_site.conv
             self.conv_flows = ConvLayer(self, sc + '/flows/conv2d/kernel', sc + '/flows/conv2d/bias', (1, 3, 3), L.WKIND_PLAIN,
-                                        (1, 1, 1), (0, 1, 1), False, hs_spec, 2 * nk)
+                                        (1, 1, 1), (0, 1, 1), False, hs_spec, 2 * self.nk)
             self.convs += [self.conv_hflow, self.conv_flows]
-            Bf['fpre'] = self._z(S, NB, H, W, hp.ngf)
-            Bf['fst'] = self._norm_stats(S, NB, hp.ngf)
-            Bf['hf'] = self._z(S, NB, H, W, hp.ngf)
-            Bf['flows'] = self._z(S, NB, H, W, _ceil4(2 * nk))
-        Bf['spre'] = self._z(S, NB, H, W, hp.ngf)
-        Bf['mpre'] = self._z(S, NB, H, W, hp.ngf)
-        Bf['sst'] = self._norm_stats(S, NB, hp.ngf)
-        Bf['mst'] = self._norm_stats(S, NB, hp.ngf)
-        Bf['hs'] = self._z(S, NB, H, W, hp.ngf)
-        Bf['mk'] = self._z(S, NB, H, W, self.mk_spec.cstride)
         self.mc = max(8, _ceil4(self.nlayers))     # channel stride of the mask logits and masks
         Bf['mlog'] = self._z(S, NB, H, W, self.mc)
         Bf['masks'] = self._z(S, NB, H, W, self.mc)
@@ -1100,10 +1142,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
                              (1, 4, 4), L.WKIND_PLAIN, (1, 2, 2), (0, 1, 1), False, spec, oc)
             self.convs.append(conv)
             Bf['epre%d' % i] = self._z(S * B, hh, ww, oc)
-            if i > 0:
+            el = dict(conv=conv, oc=oc, h=hh, w=ww)
+            if i > 0:       # layer 1 has no norm: its leaky relu runs in the convolution's epilogue, into epre0
                 Bf['eact%d' % i] = self._z(S * B, hh, ww, oc)
                 Bf['est%d' % i] = self._norm_stats(S * B, oc)
-            self.enc_layers.append(dict(conv=conv, oc=oc, h=hh, w=ww))
+                el['site'] = NormSite(self, conv, '%s/layer_%d' % (sc, i + 1), 'eact%d' % (i - 1) if i > 1 else 'epre0',
+                                      'epre%d' % i, 'est%d' % i, 'eact%d' % i, 0, S * B, L.ACT_LRELU, 0.2)
+            self.enc_layers.append(el)
             spec = ConcatSpec([('x', oc)])
         Bf['epool'] = self._z(S * B, self.enc_layers[-1]['oc'])
         Bf['zmu'] = self._z(S, B, hp.nz)
@@ -1287,16 +1332,13 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             L.broadcast_channels(Bf['actions'], A, Bf['pairs'].data_ptr() + 4 * ps.off('act'), ps.cstride, S * B, H * W, A)
         cur = Bf['pairs']
         for i, el in enumerate(self.enc_layers):
-            pre = Bf['epre%d' % i]
             if i == 0:
-                el['conv'].fwd(cur, pre, act=L.ACT_LRELU, alpha=0.2)      # networks.py:17-20
-                cur = pre
+                el['conv'].fwd(cur, Bf['epre0'], act=L.ACT_LRELU, alpha=0.2)      # networks.py:17-20
+                cur = Bf['epre0']
             else:
-                out = Bf['eact%d' % i]
-                self._site_conv(el['conv'], cur, pre, out, act=L.ACT_LRELU, alpha=0.2)
-                self._site_norm('generator/encoder/layer_%d' % (i + 1), pre, out.data_ptr(), el['oc'], S * B, el['h'] * el['w'],
-                                el['oc'], L.ACT_LRELU, 0.2, Bf['est%d' % i])
-                cur = out
+                el['site'].conv_fwd(cur, None)
+                el['site'].norm_fwd(None)
+                cur = Bf['eact%d' % i]
         last = self.enc_layers[-1]
         L.avgpool(cur, last['oc'], Bf['epool'], S * B, last['h'] * last['w'], last['oc'])
         P = self.params
@@ -1383,43 +1425,25 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         Bf = self.Bf
         S, NB, Zc = self.S, self.NB, self.Zc
         Zp = _ceil4(Zc)
-        for d in self.gl:
-            li = d['li']
-            buf = Bf['in%d' % li]
-            sp = d['in_spec']
-            if d['zin'] == 'tile':
-                L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * sp.off('z'), sp.cstride, S * NB,
-                                     buf.shape[2] * buf.shape[3], Zc)
-            if d['zr'] == 'tile':
-                buf = Bf['rin%d' % li]
-                sp = d['rin_spec']
-                L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * sp.off('z'), sp.cstride, S * NB,
-                                     buf.shape[2] * buf.shape[3], Zc)
+        for key, _, off, cs in self.ztiles:
+            buf = Bf[key]
+            L.broadcast_channels(Bf['zvec'], Zp, buf.data_ptr() + 4 * off, cs, S * NB, buf.shape[2] * buf.shape[3], Zc)
         # the sites without tile-concat: their convolution's output starts as dense(v) of its step and row, and the
         # convolution adds to it (ConvLayer.prefilled)
         for name, buf, off, c, _ in self.zdense:
             L.dense_fwd(Bf['zvec'], Zp, self.params[name], None, Bf['zw'], c, S * NB, Zc, c)
             L.broadcast_channels(Bf['zw'], c, buf.data_ptr() + 4 * off, buf.shape[-1], S * NB, buf.shape[-2] * buf.shape[-3], c)
 
-    def _h_dests(self, li, t):
-        """Where the output of generator layer li at step t must land (its consumers' concat slices)."""
-        Bf = self.Bf
-        d = self.gl[li]
-        n_enc = len(self.enc_specs)
-        dests = []
-        if d['use'] and t + 1 <= self.S and not self.hparams.ablation_rnn:
-            sp = d['rin_spec']
-            dests.append((Bf['rin%d' % li][t + 1].data_ptr() + 4 * sp.off('h'), sp.cstride))
-        if li + 1 < self.nl:
-            sp = self.gl[li + 1]['in_spec']
-            dests.append((Bf['in%d' % (li + 1)][t].data_ptr() + 4 * sp.off('x'), sp.cstride))
-        if li < n_enc - 1:       # skip connection: decoder layer n_enc + i reads layers[n_enc - i - 1]
-            i = n_enc - 1 - li
-            sp = self.gl[n_enc + i]['in_spec']
-            dests.append((Bf['in%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
-        if li == n_enc - 1 and self.cdna:     # flattened input of the CDNA kernel dense layer
-            dests.append((Bf['small'][t].data_ptr(), d['oc']))
-        return dests
+    def _addr(self, wire, t, grad=False):
+        """(address, cstride) at step t of a channel slot (Bf key, Gb key, channel offset, cstride): the forward buffer's,
+        or (grad) its gradient's."""
+        bufs = self.Gb if grad else self.Bf
+        return bufs[wire[int(grad)]][t].data_ptr() + 4 * wire[2], wire[3]
+
+    def _consumers(self, d, t, grad=False):
+        """The slots of the consumers of generator layer d's output at step t (d['wires']): where the forward copies it,
+        or (grad) the gradients the backward sums, in that order."""
+        return [self._addr(w, t, grad) for w in d['wires'] if w[int(grad)]]
 
     def _gen_step(self, t):
         hp = self.hparams
@@ -1437,57 +1461,38 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         L.copy_channels(Bf['x'][0].data_ptr(), 4, Bf['in0'][t].data_ptr() + 4 * sp.off('first'), sp.cstride, NB * HW, 4)
         for d in self.gl:
             li, oc, hh, ww = d['li'], d['oc'], d['h'], d['w']
-            pre = Bf['pre%d' % li][t]
-            site = '%s/h%d' % (sc, li)
-            if d['use']:
-                rsp = d['rin_spec']
-                rin = Bf['rin%d' % li][t]
-                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, rin, rsp.off('x'), act=self.site_act)
-                self._site_norm(site, pre, rin.data_ptr() + 4 * rsp.off('x'), rsp.cstride, NB, hh * ww, oc, self.site_act, 0.0,
-                                Bf['nst%d' % li][t])
-                b = d['rname']
-                if hp.ablation_rnn:
-                    out = Bf['out%d' % li][t]
-                    self._site_conv(d['rconv'], rin, Bf['rpre%d' % li][t], out, act=self.site_act)
-                    self._site_norm(b, Bf['rpre%d' % li][t], out.data_ptr(), oc, NB, hh * ww, oc, self.site_act, 0.0,
-                                    Bf['rnst%d' % li][t])
-                    for addr, cs in self._h_dests(li, t):
-                        L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
-                    continue
-                gpre = Bf['gpre%d' % li][t]
+            d['site'].conv_fwd(Bf['in%d' % li][t], t)
+            d['site'].norm_fwd(t)
+            if d['use'] and hp.ablation_rnn:
+                d['rsite'].conv_fwd(Bf['rin%d' % li][t], t)
+                d['rsite'].norm_fwd(t)
+            elif d['use']:
+                rin, gpre, b = Bf['rin%d' % li][t], Bf['gpre%d' % li][t], d['rname']
+                h = [self._addr(d['rec'], t + 1)]
                 if self.cell_norm:
                     d['rconv'].fwd(rin, gpre)
                     L.lstm_gates_fwd(gpre, NB, hh * ww, oc, Bf['c%d' % li][t],
                                      P[b + '/input_transform_forget_output/gamma'], P[b + '/input_transform_forget_output/beta'],
-                                     P[b + '/state/gamma'], P[b + '/state/beta'], Bf['c%d' % li][t + 1], self._h_dests(li, t),
-                                     Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t])
-                elif hp.ablation_conv_rnn_norm:
-                    dests = self._h_dests(li, t)
-                    d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], dests[:1])
-                    nm = '%s/lstm_h%d/InstanceNorm' % (sc, li)
-                    out = Bf['out%d' % li][t]
-                    L.inorm_act(dests[0][0], dests[0][1], out.data_ptr(), oc, NB, hh * ww, oc, P[nm + '/gamma'], P[nm + '/beta'],
-                                L.ACT_NONE, 0.0, Bf['hst%d' % li][t])
-                    for a, cs in dests[1:]:
-                        L.copy_channels(out.data_ptr(), oc, a, cs, NB * hh * ww, oc)
-                else:
-                    d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], self._h_dests(li, t))
-            else:
-                dests = self._h_dests(li, t)
-                out = Bf['out%d' % li][t]
-                self._site_conv(d['conv'], Bf['in%d' % li][t], pre, out, act=self.site_act)
-                self._site_norm(site, pre, out.data_ptr(), oc, NB, hh * ww, oc, self.site_act, 0.0, Bf['nst%d' % li][t])
-                for addr, cs in dests:
-                    L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
+                                     P[b + '/state/gamma'], P[b + '/state/beta'], Bf['c%d' % li][t + 1],
+                                     h + self._consumers(d, t), Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t])
+                    continue
+                if not hp.ablation_conv_rnn_norm:
+                    d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], h + self._consumers(d, t))
+                    continue
+                # the cell writes h, its instance norm the layer's output
+                d['rconv'].lstm_fwd(rin, gpre, Bf['c%d' % li][t], Bf['c%d' % li][t + 1], h)
+                nm = '%s/lstm_h%d/InstanceNorm' % (sc, li)
+                L.inorm_act(*h[0], Bf['out%d' % li][t].data_ptr(), oc, NB, hh * ww, oc, P[nm + '/gamma'], P[nm + '/beta'],
+                            L.ACT_NONE, 0.0, Bf['hst%d' % li][t])
+            out = Bf['out%d' % li][t]
+            for addr, cs in self._consumers(d, t):
+                L.copy_channels(out.data_ptr(), oc, addr, cs, NB * hh * ww, oc)
         nk, kh, kw = self.nk, self.kh, self.kw
-        top = Bf['out%d' % (self.nl - 1)][t] if not self.gl[-1]['use'] else None
-        ngf = hp.ngf
-        nl = self.nl
+        top = Bf['out%d' % (self.nl - 1)][t]
         if self.flow:
             # flow heads (savp_model.py:522-530): h_flow = relu(IN(conv3x3(top))), flows = conv3x3(h_flow) [.., 2, nk]
-            self._site_conv(self.conv_hflow, top, Bf['fpre'][t], Bf['hf'][t], act=self.site_act)
-            self._site_norm('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act, 0.0,
-                            Bf['fst'][t])
+            self.hflow_site.conv_fwd(top, t)
+            self.hflow_site.norm_fwd(t)
             self.conv_flows.fwd(Bf['hf'][t], Bf['flows'][t], out_c=2 * nk)
         elif self.cdna:
             # cdna kernels (savp_model.py:546-559)
@@ -1497,19 +1502,14 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
             L.dense_fwd(small, K, P[sc + '/cdna_kernels/dense/kernel'], P[sc + '/cdna_kernels/dense/bias'], Bf['kraw'][t],
                         kh * kw * nk, NB, K, kh * kw * nk, k_splits=32)
             L.cdna_kernel_norm(Bf['kraw'][t], Bf['kern'][t], NB, kh, kw, nk)
-        # heads
+        # heads: both convolutions, then both norms
         mk = Bf['mk'][t]
         msp = self.mk_spec
-        if self.conv_scratch:
-            self._site_conv(self.conv_scratch, top, Bf['spre'][t], Bf['hs'][t], act=self.site_act)
-        if self.conv_hmasks:
-            self._site_conv(self.conv_hmasks, top, Bf['mpre'][t], mk, msp.off('hm'), act=self.site_act)
-        if self.conv_scratch:
-            self._site_norm('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf, NB, HW, ngf, self.site_act,
-                            0.0, Bf['sst'][t])
-        if self.conv_hmasks:
-            self._site_norm('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride, NB, HW, ngf,
-                            self.site_act, 0.0, Bf['mst'][t])
+        heads = [s for s in (self.scratch_site, self.hmasks_site) if s]
+        for s in heads:
+            s.conv_fwd(top, t)
+        for s in heads:
+            s.norm_fwd(t)
         if self.conv_simg:      # scratch image -> last layer slot (savp_model.py:570-572, 595-596)
             self.conv_simg.fwd(Bf['hs'][t], mk, out_off=msp.off('l%d' % (self.nlayers - 1)), out_c=C, act=L.ACT_SIGMOID)
         # transformed images of the history, then the backgrounds (savp_model.py:574-594)
@@ -1556,26 +1556,29 @@ class SAVPVideoPredictionModel(TrainMixin, VideoPredictionModel):
         src = {'prev': self.Bf['img'][t], 'first': x[0], 'last': x[ctx - 1], 'last_context': x[t if t < ctx else ctx - 1]}
         return [(x[b[1]] if isinstance(b, tuple) else src[b]).data_ptr() for b in self.comp['bgs']]
 
+    def _initial_state_slot(self, what, li, grad=False):
+        """Where the learned initial state (what, li) of _initial_state_specs is tiled to, or (grad) where its gradient is
+        summed from: the t = 0 state buffer c[0], zc[0], zh[0] or, for a ConvLSTM's h, the contiguous h0 buffer; then, for
+        h, the strided h slot (d['rec']) that h0 is copied into / from, else None."""
+        bufs, p = (self.Gb, 'd') if grad else (self.Bf, '')
+        if what == 'h':
+            return bufs[p + 'h0_%d' % li], self.gl[li]['rec']
+        return bufs[p + ('c%d' % li if what == 'c' else what)][0], None
+
     def _load_initial_states(self, conv):
         """The learned initial states (learn_initial_state), tiled over the NB rows into the t = 0 state buffers: the ConvLSTMs'
         c[0] and the h slot of rin[0] (conv=True), or the z cell's zc[0] / zh[0] (conv=False).  Runs inside the step, so that a
         captured graph reads the variables Adam has updated."""
-        Bf, NB = self.Bf, self.NB
         for name, _, what, li in self._initial_state_specs():
             if what.startswith('z') == conv:
                 continue
             v = self.params[name]
             n = v.numel()
-            if what in ('zc', 'zh', 'c'):
-                dst = Bf[what if what != 'c' else 'c%d' % li][0]
-                L.copy_channels(v.data_ptr(), 0, dst.data_ptr(), n, NB, n)
-                continue
-            d = self.gl[li]
-            sp = d['rin_spec']
-            h0 = Bf['h0_%d' % li]        # tiled [NB, hh, ww, oc], then into the strided h slot
-            L.copy_channels(v.data_ptr(), 0, h0.data_ptr(), n, NB, n)
-            L.copy_channels(h0.data_ptr(), d['oc'], Bf['rin%d' % li][0].data_ptr() + 4 * sp.off('h'), sp.cstride,
-                            NB * d['h'] * d['w'], d['oc'])
+            dst, h_slot = self._initial_state_slot(what, li)
+            L.copy_channels(v.data_ptr(), 0, dst.data_ptr(), n, self.NB, n)
+            if h_slot:
+                d = self.gl[li]
+                L.copy_channels(dst.data_ptr(), d['oc'], *self._addr(h_slot, 0), self.NB * d['h'] * d['w'], d['oc'])
 
     def generator_forward(self, collect=True):
         hp = self.hparams

@@ -363,7 +363,7 @@ class TrainMixin(object):
         HW = H * W
         S = self.S
         sc = 'generator/rnn/savp_cell'
-        nl, ngf = self.nl, hp.ngf
+        ngf = hp.ngf
         msp = self.mk_spec
         mk, dmk = Bf['mk'][t], G['dmk'][t]
         nlay = self.nlayers
@@ -374,10 +374,7 @@ class TrainMixin(object):
         if self.conv_masks:
             self.conv_masks.dgrad(G['dmlog'][t], dmk, dy_c=nlay)
             # h_masks branch
-            self._site_norm_bwd('%s/h%d_masks' % (sc, nl), Bf['mpre'][t], mk.data_ptr() + 4 * msp.off('hm'), msp.cstride,
-                                [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dmpre'][t], NB, HW, ngf, self.site_act, 0.0,
-                                Bf['mst'][t])
-            self.conv_hmasks.dgrad(G['dmpre'][t], G['dtop'][t])
+            self.hmasks_site.bwd(t, [(dmk.data_ptr() + 4 * msp.off('hm'), msp.cstride)], G['dtop'][t])
             dtop_acc = True
         if self.conv_scratch:
             # scratch branch
@@ -385,9 +382,7 @@ class TrainMixin(object):
             L.act_bwd(mk.data_ptr() + 4 * so, msp.cstride, dmk.data_ptr() + 4 * so, msp.cstride,
                       G['dlay'][t].data_ptr() + 4 * 4 * (nlay - 1), 4 * nlay, G['dsimg'][t].data_ptr(), 4, NB * HW, C, L.ACT_SIGMOID)
             self.conv_simg.dgrad(G['dsimg'][t], G['dhs'][t], dy_c=C)
-            self._site_norm_bwd('%s/h%d_scratch' % (sc, nl), Bf['spre'][t], Bf['hs'][t].data_ptr(), ngf,
-                                [(G['dhs'][t].data_ptr(), ngf)], G['dspre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['sst'][t])
-            self.conv_scratch.dgrad(G['dspre'][t], G['dtop'][t], accumulate=dtop_acc)
+            self.scratch_site.bwd(t, [(G['dhs'][t].data_ptr(), ngf)], G['dtop'][t], accumulate=dtop_acc)
             dtop_acc = True
         nk, kh, kw = self.nk, self.kh, self.kw
         # transforms and the previous-image background -> the history images (dimg[s], zeroed once per backward, so that
@@ -399,9 +394,7 @@ class TrainMixin(object):
             L.slots_bwd(frames, nk, self.comp['prev_slot'], *da, dframes, NB, H, W, flows=Bf['flows'][t], flows_cs=Bf['flows'].shape[-1],
                         dflows=G['dflows'][t])
             self.conv_flows.dgrad(G['dflows'][t], G['dhf'][t], dy_c=2 * nk)
-            self._site_norm_bwd('%s/h%d_flow' % (sc, nl), Bf['fpre'][t], Bf['hf'][t].data_ptr(), ngf, [(G['dhf'][t].data_ptr(), ngf)],
-                                G['dfpre'][t], NB, HW, ngf, self.site_act, 0.0, Bf['fst'][t])
-            self.conv_hflow.dgrad(G['dfpre'][t], G['dtop'][t], accumulate=dtop_acc)
+            self.hflow_site.bwd(t, [(G['dhf'][t].data_ptr(), ngf)], G['dtop'][t], accumulate=dtop_acc)
             dtop_acc = True
         elif not self.cdna:
             L.slots_bwd(frames, 0, self.comp['prev_slot'], *da, dframes, NB, H, W)
@@ -418,64 +411,37 @@ class TrainMixin(object):
                         dx_stride=K)
         if not dtop_acc:        # no head reads the top layer
             G['dtop'][t].zero_()
-        # encoder/decoder stack in reverse
-        n_enc = len(self.enc_specs)
-        for li in range(nl - 1, -1, -1):
-            d = self.gl[li]
-            oc, hh, ww = d['oc'], d['h'], d['w']
-            srcs = []
-            if li == nl - 1:
-                srcs.append((G['dtop'][t].data_ptr(), oc))
-            else:
-                sp = self.gl[li + 1]['in_spec']
-                srcs.append((G['din%d' % (li + 1)][t].data_ptr() + 4 * sp.off('x'), sp.cstride))
-            if li < n_enc - 1:
-                i = n_enc - 1 - li
-                sp = self.gl[n_enc + i]['in_spec']
-                srcs.append((G['din%d' % (n_enc + i)][t].data_ptr() + 4 * sp.off('skip'), sp.cstride))
-            if li == n_enc - 1 and self.cdna:
-                srcs.append((G['dsmall'][t].data_ptr(), oc))
+        # encoder/decoder stack in reverse: each layer's output gradient is the sum of its consumers' (_consumers), then
+        # for a ConvLSTM that of its h slot at step t + 1
+        for d in reversed(self.gl):
+            li, oc, hh, ww = d['li'], d['oc'], d['h'], d['w']
+            srcs = self._consumers(d, t, grad=True)
+            rec = [self._addr(d['rec'], t + 1, grad=True)] if 'rec' in d and t + 1 < S else []
             if d['use'] and hp.ablation_rnn:
-                # the conv_h site: its output's gradient through norm + activation and the 5x5 conv to (h{li} | z)
-                rsp = d['rin_spec']
-                self._site_norm_bwd(d['rname'], Bf['rpre%d' % li][t], Bf['out%d' % li][t].data_ptr(), oc, srcs, G['drpre%d' % li][t],
-                                    NB, hh * ww, oc, self.site_act, 0.0, Bf['rnst%d' % li][t])
-                d['rconv'].dgrad(G['drpre%d' % li][t], G['drin%d' % li][t])
-                srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
+                d['rsite'].bwd(t, srcs, G['drin%d' % li][t])
             elif d['use'] and not self.cell_norm:
-                rsp = d['rin_spec']
                 if 'hst%d' % li in Bf:    # h -> IN(h) -> consumers: their gradient through the norm, before the recurrent one
                     nm_h = '%s/lstm_h%d/InstanceNorm' % (sc, li)
-                    L.inorm_act_bwd(Bf['rin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride, srcs,
-                                    G['dhn%d' % li][t].data_ptr(), oc, NB, hh * ww, oc, P[nm_h + '/gamma'], P[nm_h + '/beta'],
-                                    Bf['hst%d' % li][t], L.ACT_NONE, 0.0, Gp[nm_h + '/gamma'], Gp[nm_h + '/beta'])
+                    L.inorm_act_bwd(*self._addr(d['rec'], t + 1), srcs, G['dhn%d' % li][t].data_ptr(), oc, NB, hh * ww, oc,
+                                    P[nm_h + '/gamma'], P[nm_h + '/beta'], Bf['hst%d' % li][t], L.ACT_NONE, 0.0,
+                                    Gp[nm_h + '/gamma'], Gp[nm_h + '/beta'])
                     srcs = [(G['dhn%d' % li][t].data_ptr(), oc)]
-                if t + 1 < S:
-                    srcs.append((G['drin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride))
-                L.lstm_plain_bwd(Bf['gpre%d' % li][t], Bf['c%d' % li][t], Bf['c%d' % li][t + 1], NB * hh * ww, oc, srcs,
+                L.lstm_plain_bwd(Bf['gpre%d' % li][t], Bf['c%d' % li][t], Bf['c%d' % li][t + 1], NB * hh * ww, oc, srcs + rec,
                                  G['dc%d' % li][t + 1] if t + 1 < S else None, G['dgpre%d' % li][t], G['dc%d' % li][t])
                 d['rconv'].dgrad(G['dgpre%d' % li][t], G['drin%d' % li][t])
-                srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
             elif d['use']:
-                rsp = d['rin_spec']
-                if t + 1 < S:
-                    srcs.append((G['drin%d' % li][t + 1].data_ptr() + 4 * rsp.off('h'), rsp.cstride))
                 b = d['rname']
                 L.lstm_gates_bwd(Bf['gpre%d' % li][t], NB, hh * ww, oc, Bf['c%d' % li][t],
                                  P[b + '/input_transform_forget_output/gamma'], P[b + '/input_transform_forget_output/beta'],
-                                 P[b + '/state/gamma'], P[b + '/state/beta'], Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t], srcs,
-                                 G['dc%d' % li][t + 1] if t + 1 < S else None, G['dgpre%d' % li][t], G['dc%d' % li][t],
+                                 P[b + '/state/gamma'], P[b + '/state/beta'], Bf['gst1_%d' % li][t], Bf['gst2_%d' % li][t],
+                                 srcs + rec, G['dc%d' % li][t + 1] if t + 1 < S else None, G['dgpre%d' % li][t], G['dc%d' % li][t],
                                  Gp[b + '/input_transform_forget_output/gamma'], Gp[b + '/input_transform_forget_output/beta'],
                                  Gp[b + '/state/gamma'], Gp[b + '/state/beta'])
                 d['rconv'].dgrad(G['dgpre%d' % li][t], G['drin%d' % li][t])
+            if d['use']:         # the h{li} site's output is the 'x' slot of the recurrent site's input
+                rsp = d['rin_spec']
                 srcs = [(G['drin%d' % li][t].data_ptr() + 4 * rsp.off('x'), rsp.cstride)]
-            if d['use']:         # the site's output: the 'x' slot of the ConvLSTM's input, or the layer's own buffer
-                y_addr, y_cs = Bf['rin%d' % li][t].data_ptr() + 4 * d['rin_spec'].off('x'), d['rin_spec'].cstride
-            else:
-                y_addr, y_cs = Bf['out%d' % li][t].data_ptr(), oc
-            self._site_norm_bwd('%s/h%d' % (sc, li), Bf['pre%d' % li][t], y_addr, y_cs, srcs, G['dpre%d' % li][t], NB, hh * ww, oc,
-                                self.site_act, 0.0, Bf['nst%d' % li][t])
-            d['conv'].dgrad(G['dpre%d' % li][t], G['din%d' % li][t])
+            d['site'].bwd(t, srcs, G['din%d' % li][t])
         # gradient w.r.t. the input image of this step: CDNA path + first conv's 'image' slot
         sp = self.gl[0]['in_spec']
         L.axpy_channels(G['din0'][t].data_ptr() + 4 * sp.off('image'), sp.cstride, G['dimg'][t].data_ptr(), 4, NB * HW, 4)
@@ -505,32 +471,26 @@ class TrainMixin(object):
             self._initial_state_grads(conv=True)
         if self.Zc:
             G['dzvec'].zero_()
-        zdense = {s[4]: s for s in self.zdense}
         for d in self.gl:
             li = d['li']
-            for key in ('dpre%d' % li, 'drpre%d' % li, 'dgpre%d' % li):
-                if key in zdense:
-                    self._zdense_backward(*zdense[key])
-            d['conv'].wgrad(Bf['in%d' % li], G['dpre%d' % li])
-            L.colsum(G['dpre%d' % li].data_ptr(), d['oc'], Gp[d['conv'].bname], 1, S * NB * d['h'] * d['w'], d['oc'])
-            if d['use']:
-                dy = G['drpre%d' % li] if hp.ablation_rnn else G['dgpre%d' % li]
+            for z in d['zdense']:       # the layer's dense terms, h{li} first, before its weight gradients
+                self._zdense_backward(*z)
+            d['site'].param_grads()
+            if d['use'] and hp.ablation_rnn:
+                d['rsite'].param_grads()
+            elif d['use']:
+                dy = G['dgpre%d' % li]
                 d['rconv'].wgrad(Bf['rin%d' % li][:S], dy)
-                if d['rconv'].bname:      # norm-free cell / conv_h site: the convolution's bias
+                if d['rconv'].bname:      # norm-free cell: the convolution's bias
                     L.colsum(dy.data_ptr(), dy.shape[-1], Gp[d['rconv'].bname], 1, S * NB * d['h'] * d['w'], dy.shape[-1])
             if red is not None:
                 pre = ('%s/h%d/' % (sc_cell, li), '%s/lstm_h%d/' % (sc_cell, li), '%s/conv_h%d/' % (sc_cell, li))
                 lo, hi = self._flat_range(self.g_flat, [k for k in P if k.startswith(pre)])
                 red.reduce_range(self.g_grad, lo, hi)
                 done.append((lo, hi))
-        top = Bf['out%d' % (self.nl - 1)]
-        ngf = hp.ngf
-        if self.conv_scratch:
-            self.conv_scratch.wgrad(top, G['dspre'])
-            L.colsum(G['dspre'].data_ptr(), ngf, Gp[self.conv_scratch.bname], 1, rows_top, ngf)
-        if self.conv_hmasks:
-            self.conv_hmasks.wgrad(top, G['dmpre'])
-            L.colsum(G['dmpre'].data_ptr(), ngf, Gp[self.conv_hmasks.bname], 1, rows_top, ngf)
+        for s in (self.scratch_site, self.hmasks_site):
+            if s:
+                s.param_grads()
         if self.conv_simg:
             self.conv_simg.wgrad(Bf['hs'], G['dsimg'], dy_c=C)
             L.colsum(G['dsimg'].data_ptr(), 4, Gp[self.conv_simg.bname], 1, rows_top, C)
@@ -538,8 +498,7 @@ class TrainMixin(object):
             self.conv_masks.wgrad(Bf['mk'], G['dmlog'], dy_c=self.nlayers)
             L.colsum(G['dmlog'].data_ptr(), self.mc, Gp[self.conv_masks.bname], 1, rows_top, self.nlayers)
         if self.flow:
-            self.conv_hflow.wgrad(top, G['dfpre'])
-            L.colsum(G['dfpre'].data_ptr(), ngf, Gp[self.conv_hflow.bname], 1, rows_top, ngf)
+            self.hflow_site.param_grads()
             self.conv_flows.wgrad(Bf['hf'], G['dflows'], dy_c=2 * self.nk)
             L.colsum(G['dflows'].data_ptr(), G['dflows'].shape[-1], Gp[self.conv_flows.bname], 1, rows_top, 2 * self.nk)
         elif self.cdna:
@@ -552,14 +511,9 @@ class TrainMixin(object):
             return
         # tile_concat adjoint: sum the z-slot gradients of every concat buffer over space
         Zc, Zp = self.Zc, _ceil4(self.Zc)
-        for d in self.gl:
-            li = d['li']
-            for key, spn, form in (('din%d' % li, 'in_spec', d['zin']), ('drin%d' % li, 'rin_spec', d['zr'])):
-                if form != 'tile':
-                    continue
-                buf = G[key][:S]
-                sp = d[spn]
-                L.colsum(buf.data_ptr() + 4 * sp.off('z'), sp.cstride, G['dzvec'], S * NB, buf.shape[2] * buf.shape[3], Zc, out_stride=Zp)
+        for _, key, off, cs in self.ztiles:
+            buf = G[key]
+            L.colsum(buf.data_ptr() + 4 * off, cs, G['dzvec'], S * NB, buf.shape[2] * buf.shape[3], Zc, out_stride=Zp)
         if not hp.nz:
             return
         # the action and state slots' gradients are discarded: the states enter under stop_gradient (savp_model.py:414-421)
@@ -613,19 +567,14 @@ class TrainMixin(object):
                 dact = G['deact%d' % i] if i > 0 else G['depre0']
                 L.avgpool_bwd(G['depool'], dact, oc, S * B, pos, oc)
             if i > 0:
-                self._site_norm_bwd('%s/layer_%d' % (sc, i + 1), Bf['epre%d' % i], Bf['eact%d' % i].data_ptr(), oc,
-                                    [(G['deact%d' % i].data_ptr(), oc)], G['depre%d' % i], S * B, pos, oc, L.ACT_LRELU, 0.2,
-                                    Bf['est%d' % i])
-                x_in = Bf['eact%d' % (i - 1)] if i > 1 else Bf['epre0']
-                dst = G['deact%d' % (i - 1)] if i > 1 else G['depre0']
-                el['conv'].dgrad(G['depre%d' % i], dst)
-            else:
-                # layer 1 stored the lrelu OUTPUT (activation fused in the conv epilogue)
-                L.act_bwd(Bf['epre0'].data_ptr(), oc, G['depre0'].data_ptr(), oc, 0, oc, G['depre0'].data_ptr(), oc, S * B * pos, oc,
-                          L.ACT_LRELU, 0.2)
-                x_in = Bf['pairs']
-            el['conv'].wgrad(x_in, G['depre%d' % i])
-            L.colsum(G['depre%d' % i].data_ptr(), oc, Gp[el['conv'].bname], 1, S * B * pos, oc)
+                el['site'].bwd(None, [(G['deact%d' % i].data_ptr(), oc)], G['deact%d' % (i - 1)] if i > 1 else G['depre0'])
+                el['site'].param_grads()
+                continue
+            # layer 1 stored the lrelu OUTPUT (activation fused in the conv epilogue)
+            L.act_bwd(Bf['epre0'].data_ptr(), oc, G['depre0'].data_ptr(), oc, 0, oc, G['depre0'].data_ptr(), oc, S * B * pos, oc,
+                      L.ACT_LRELU, 0.2)
+            el['conv'].wgrad(Bf['pairs'], G['depre0'])
+            L.colsum(G['depre0'].data_ptr(), oc, Gp[el['conv'].bname], 1, S * B * pos, oc)
 
     def _zdense_backward(self, name, buf, off, c, dy):
         """The dense term of a site without tile-concat (out = conv(h) + dense(v, W)): its output gradient summed over space
@@ -642,19 +591,15 @@ class TrainMixin(object):
     def _initial_state_grads(self, conv):
         """Gradients of the learned initial states: the sum over the NB rows of the t = 0 state gradient -- dc[0] and the h
         slot of drin[0] of the ConvLSTMs (conv=True), dzc[0] / dzh[0] of the z cell (conv=False)."""
-        G, Gp, NB = self.Gb, self.grads, self.NB
+        Gp, NB = self.grads, self.NB
         for name, _, what, li in self._initial_state_specs():
             if what.startswith('z') == conv:
                 continue
             n = self.params[name].numel()
-            if what in ('zc', 'zh', 'c'):
-                src = G['d' + what if what != 'c' else 'dc%d' % li][0]
-            else:
+            src, h_slot = self._initial_state_slot(what, li, grad=True)
+            if h_slot:      # the strided h slot made contiguous per row
                 d = self.gl[li]
-                sp = d['rin_spec']
-                src = G['dh0_%d' % li]       # the strided h slot made contiguous per row
-                L.copy_channels(G['drin%d' % li][0].data_ptr() + 4 * sp.off('h'), sp.cstride, src.data_ptr(), d['oc'],
-                                NB * d['h'] * d['w'], d['oc'])
+                L.copy_channels(*self._addr(h_slot, 0, grad=True), src.data_ptr(), d['oc'], NB * d['h'] * d['w'], d['oc'])
             L.colsum(src.data_ptr(), n, Gp[name], 1, NB, n)
 
     def _gru_z_backward(self):
